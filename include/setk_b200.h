@@ -324,6 +324,39 @@ int64_t setk_msc_work_doubles(int32_t T, int32_t F);
 int setk_msc(const void* spec, int32_t N, int32_t T, int32_t F, int32_t context, int32_t normalize,
              double* work, double* out, void* stream);
 
+/* ---- sound source localisation on explicit STFTs: scripts/sptk/libs/ssl.py, do_ssl.py ---- */
+#define SETK_SSL_ML 0           /* ml_ssl    ssl.py:12-43 (do_ssl.py:34 passes compression=-1, eps=EPSILON) */
+#define SETK_SSL_SRP 1          /* srp_ssl   ssl.py:46-77 */
+#define SETK_SSL_MUSIC 2        /* music_ssl ssl.py:80-110 */
+#define SETK_SSL_MAX_MASKS 8
+
+/*
+ * DoA scores and their arg-extreme for every (utterance, mask, frame window, direction).
+ *   backend      SETK_SSL_*
+ *   stft         c64 [B][M][F][T]     (the reference's M x T x F per utterance, bins before frames here)
+ *   steer        c128 [A][M][steer_F] steering vectors as np.load gives them (compute_steer_vector.py:44-51,
+ *                do_ssl.py:49); ML normalises them over microphones (ssl.py:27), MUSIC uses them as given
+ *   steer_F      bins of the steering table: SETK_ESHAPE unless it equals F
+ *   mask         f32 [B][N][T][F] or NULL (ssl.py:24-25,58-61,91-92: all ones); N > 1 is the 3-D mask of
+ *                ml_ssl (ssl.py:41-42), ML only, N <= SETK_SSL_MAX_MASKS; N must be 1 when mask is NULL
+ *   windows_host i32 [B][W][2] HOST array of frame ranges [s, e), 0 <= s < e <= T: [0, T) offline, the
+ *                chunks [max(t - look_back, 0), t + chunk_len) of do_ssl.py's online mode (:103-111)
+ *   pairs_host   i32 [P][2] HOST array of microphone pairs (l, r), SRP only (srp_pair, ssl.py:62; do_ssl.py:70-74)
+ *   compression  ML: <= 0 -> -log(max(delta, eps)), else -delta**compression (ssl.py:34-37)
+ *   eps          ML: floor of delta and of |x| for normalize, delta = ssh - ssv / (1 + eps) (ssl.py:29,33)
+ *   normalize    ML: x / max(|x|, eps) first (norm=True, ssl.py:28-29)
+ *   scores       f64 [B][N][W][A]: ML the masked log-likelihood sum (ssl.py:39-42), SRP the masked mean
+ *                pair response (:71-76), MUSIC sum_f |s^H (I - u u^H) s| (:93-109)
+ *   index        i32 [B][N][W]: numpy's argmax of the scores (ML, SRP) or argmin (MUSIC) -- the first
+ *                extreme, or the first NaN when there is one
+ * Plan-free; scratch is stream-ordered.  SETK_EINVAL for an unknown backend, N > 1 with SRP or MUSIC, a
+ * pair index outside [0, M), A < 1, a window outside [0, T] or empty, M > SETK_MAX_CHANNELS.
+ */
+int setk_ssl(int32_t backend, const void* stft, int32_t B, int32_t M, int32_t F, int32_t T, const void* steer,
+             int32_t A, int32_t steer_F, const float* mask, int32_t N, const int32_t* windows_host, int32_t W,
+             const int32_t* pairs_host, int32_t P, double compression, double eps, int32_t normalize,
+             double* scores, int32_t* index, void* stream);
+
 /* floor(y * 32768) clipped to int16: the PCM_16 conversion of
  * WaveWriter.write -> write_wav -> soundfile (data_handler.py:600-605,
  * utils.py:45-62; SURVEY.md finding 3).  wave f32 [n], pcm i16 [n]. */

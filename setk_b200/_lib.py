@@ -28,6 +28,8 @@ BF_MVDR, BF_MPDR, BF_MPDR_WHITEN, BF_GEVD, BF_PMWF, BF_PEVD = 0, 1, 2, 3, 4, 5
 RANK1_NONE, RANK1_EIG, RANK1_GEV = 0, 1, 2
 F_CLIP_MASK, F_MASK_FT = 1, 2
 C64, C128 = 0, 1
+SSL_ML, SSL_SRP, SSL_MUSIC = 0, 1, 2
+SSL_MAX_MASKS = 8
 
 
 class SetkConfig(Structure):
@@ -101,6 +103,9 @@ _PROTOTYPES = {
     "setk_float_to_pcm16": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),
     "setk_pcm16_to_float": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),
     "setk_cm_masks": (c_int, [c_void_p, c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
+    "setk_ssl": (c_int, [c_int32, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_int32, c_int32,
+                         c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_int32, c_double, c_double, c_int32,
+                         c_void_p, c_void_p, c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)

@@ -270,3 +270,144 @@ def df_on_mask_main(argv=None):
             yield key, directional_feats(obs, steer.transpose(0, 1), df_pair=pairs)
 
     _dump_archive(args.dup_ark, args.scp, items(), "DF")
+
+
+# ---------------------------------------------------------------------------------------------
+# do_ssl.py (reference: add_wta :17-27, get_doa :30-37, run :40-115, flags :118-172)
+# ---------------------------------------------------------------------------------------------
+def add_wta(masks_list, eps=1e-4):
+    """Winner-take-all masks (do_ssl.py:17-27): a cell keeps its value where it is the largest."""
+    top = np.max(np.stack(masks_list, axis=-1), -1)
+    return [np.where(m == top, m, eps) for m in masks_list]
+
+
+def ssl_windows(T, chunk_len, look_back):
+    """
+    Frame windows of do_ssl.py: [0, T) offline; online (chunk_len > 0 and look_back > 0) the chunks
+    [max(t - look_back, 0), min(t + chunk_len, T)) for t = 0, chunk_len, ... (:63,103-109).
+    """
+    if chunk_len > 0 and look_back > 0:
+        return [(max(t - look_back, 0), min(t + chunk_len, T)) for t in range(0, T, chunk_len)]
+    return [(0, T)]
+
+
+def ssl_main(argv=None):
+    """
+    Sound source localisation with ML / SRP / MUSIC, optionally informed by TF-masks.
+
+    One deliberate difference from the reference: in online mode with a mask, do_ssl.py:106
+    slices mask[..., s:t + chunk_len] after the mask has become T x F, i.e. it cuts FREQUENCY
+    bins, and ml_ssl then fails with a broadcast ValueError.  Here every chunk uses the mask's
+    frames s .. t + chunk_len - 1, the same frames as its STFT chunk.
+    """
+    from . import plan as _plan
+    from .libs.data_handler import NumpyReader
+    from .libs.utils import EPSILON, default_device
+    args = _parser(
+        "Command to ML/SRP based sound souce localization (SSL).Also see scripts/sptk/compute_steer_vector.py",
+        [("wav_scp", "Multi-channel wave rspecifier"),
+         ("steer_vector", "Pre-computed steer vector in each directions (in shape A x M x F, A: number of "
+                          "DoAs, M: microphone number, F: FFT bins)"),
+         ("doa_scp", "Wspecifier for estimated DoA")],
+        [("--backend", str, "ml", None, "Which algorithm to choose for SSL (ml | srp | music)"),
+         ("--srp-pair", str, "", None, "Microphone index pair to compute srp response"),
+         ("--doa-range", str, "0,360", None, "DoA range"),
+         ("--mask-scp", str, "", None, "Rspecifier for TF-masks in numpy format"),
+         ("--output", str, "degree", None, "Output type of the DoA (radian | degree | index)"),
+         ("--mask-eps", float, -1, None, "Value of eps used in masking winner-take-all"),
+         ("--chunk-len", int, -1, None, "Number frames per chunk (for online setups)"),
+         ("--look-back", int, 125, None, "Number of frames to look back (for online setups)")]).parse_args(argv)
+    if args.backend not in ("ml", "srp", "music"):
+        raise SystemExit(f"--backend: invalid choice {args.backend!r}")
+    if args.output not in ("radian", "degree", "index"):
+        raise SystemExit(f"--output: invalid choice {args.output!r}")
+    steer_vector = np.load(args.steer_vector)
+    logger.info(f"Shape of the steer vector: {steer_vector.shape}")
+    num_doa = steer_vector.shape[0]
+    min_doa, max_doa = str2tuple(args.doa_range)
+    if args.output == "radian":
+        angles = np.linspace(min_doa * np.pi / 180, max_doa * np.pi / 180, num_doa + 1)
+    else:
+        angles = np.linspace(min_doa, max_doa, num_doa + 1)
+    reader = SpectrogramReader(args.wav_scp, **_stft_options(args, transpose=False))
+    mask_reader = [NumpyReader(scp) for scp in args.mask_scp.split(",")] if args.mask_scp else None
+    online = args.chunk_len > 0 and args.look_back > 0
+    if online:
+        logger.info(f"Set up in online mode: chunk_len = {args.chunk_len}, look_back = {args.look_back}")
+    pairs = None
+    if args.backend == "srp":
+        pairs = _pairs(args.srp_pair, "--srp-pair")
+        logger.info(f"Choose srp-based algorithm, srp pair is "
+                    f"{([p[0] for p in pairs], [p[1] for p in pairs])}")
+    steer = torch.as_tensor(steer_vector, device=default_device()).to(torch.complex128)
+    kw = dict(compression=-1, eps=EPSILON) if args.backend == "ml" else {}
+
+    def label(i):
+        return float(i) if args.output == "index" else angles[i]
+
+    done = 0
+    with open(args.doa_scp, "w") as doa_out:
+        for key, _, S in _each_stft(reader):               # S: M x F x T on the device
+            _, F, T = S.shape
+            mask = None
+            if mask_reader:
+                mask = [r[key] for r in mask_reader]
+                if args.mask_eps >= 0 and len(mask_reader) > 1:
+                    mask = add_wta(mask, eps=args.mask_eps)
+                mask = mask[0]
+                if mask.shape[-1] != F:                     # F x T => T x F
+                    mask = mask.transpose()
+                mask = torch.from_numpy(np.ascontiguousarray(mask, dtype=np.float32))[None, None]
+            windows = ssl_windows(T, args.chunk_len, args.look_back)
+            _, index = _plan.ssl(S[None], steer, backend=args.backend, mask=mask, windows=[windows],
+                                 pairs=pairs, **kw)
+            doa = [label(i) for i in index[0, 0].cpu().tolist()]
+            if not online:
+                logger.info(f"Processing utterance {key}: {doa[0]:.4f}")
+                doa_out.write(f"{key}\t{doa[0]:.4f}\n")
+            else:
+                logger.info(f"Processing utterance {key}...")
+                doa_out.write(f"{key}\t" + " ".join(f"{d:.4f}" for d in doa) + "\n")
+            done += 1
+    logger.info(f"Processing {done} utterance done")
+
+
+# ---------------------------------------------------------------------------------------------
+# compute_steer_vector.py (reference: run :17-51, flags :54-105)
+# ---------------------------------------------------------------------------------------------
+def steer_vector_main(argv=None):
+    """
+    Steering vectors A x M x F (complex128 .npy) of a linear or circular array.  Geometry
+    constants computed on the host with numpy, like the fixed beamformers' weights.
+    """
+    from .libs.beamformer import circular_steer_vector, linear_steer_vector
+    p = argparse.ArgumentParser(description="Command to compute steer vectors, using for SSL & BF & AF computation",
+                                formatter_class=argparse.ArgumentDefaultsHelpFormatter)
+    p.add_argument("steer_vector", type=str, help="Output location of the steer vector")
+    for name, typ, default, text in (
+            ("--num-doas", int, 181, "Step size when sampling the DoA"),
+            ("--num-bins", int, 257, "Number of the FFT points used"),
+            ("--sr", int, 16000, "Sample rate of input wave"),
+            ("--speed", float, 343, "Speed of sound"),
+            ("--linear-topo", str2tuple, (), "Topology of linear microphone arrays"),
+            ("--circular-around", int, 6, "Number of the micriphones in circular arrays"),
+            ("--circular-radius", float, 0.05, "Radius of circular array"),
+            ("--circular-center", strtobool, False, "Is there a microphone put in the center of the circular array?"),
+            ("--geometry", str, "linear", "Geometry of the microphone array (linear | circular)"),
+            ("--normalize", strtobool, False, "Normalzed steer vector or not")):
+        p.add_argument(name, type=typ, default=default, help=text)
+    args = p.parse_args(argv)
+    if args.geometry not in ("linear", "circular"):
+        raise SystemExit(f"--geometry: invalid choice {args.geometry!r}")
+    if args.geometry == "linear":
+        topo = np.array(args.linear_topo)
+        candidate_doa = np.linspace(0, 180, args.num_doas)
+        sv = [linear_steer_vector(topo, doa, args.num_bins, c=args.speed, sr=args.sr) for doa in candidate_doa]
+    else:
+        candidate_doa = np.arange(0, 360, 360 / args.num_doas)
+        sv = [circular_steer_vector(args.circular_radius, args.circular_around, doa, args.num_bins, c=args.speed,
+                                    sr=args.sr, center=args.circular_center) for doa in candidate_doa]
+    sv = np.stack(sv)                                       # A x F x M
+    if args.normalize:
+        sv = sv / sv.shape[-1]**0.5
+    np.save(args.steer_vector, sv.transpose(0, 2, 1))       # A x M x F

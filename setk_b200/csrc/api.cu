@@ -68,6 +68,9 @@ cudaError_t run_stft_spill(setk_plan*, const float*, const int*, int, int, int, 
 cudaError_t run_cov_spill(setk_plan*, const float2*, const float*, const float*, unsigned, const int*,
                           int, int, int, int, float*, float2*, float2*, void*);
 cudaError_t run_bits_to_float(const unsigned*, int, float*, void*);
+size_t ssl_scratch_bytes(int, int, int, int, int, int, int, int, int);
+cudaError_t run_ssl(int, const float2*, int, int, int, int, const double2*, int, const float*, int, const int*,
+                    int, const int*, int, double, double, int, char*, double*, int*, void*);
 
 struct WeightsArgs;
 cudaError_t weights_run(int kind, double beta, int ref_channel, int rank1, int ban, const void* Rs,
@@ -663,6 +666,47 @@ int setk_msc(const void* spec, int32_t N, int32_t T, int32_t F, int32_t context,
   if (context < 0) return fail(SETK_EINVAL, "setk_msc: context %d < 0", context);
   cudaError_t e = run_msc(static_cast<const float2*>(spec), N, T, F, context, normalize, work, out, stream);
   return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_msc");
+}
+
+// ---- sound source localisation (ssl.cuh, built in spatial.cu) ----
+int setk_ssl(int32_t backend, const void* stft, int32_t B, int32_t M, int32_t F, int32_t T, const void* steer,
+             int32_t A, int32_t steer_F, const float* mask, int32_t N, const int32_t* windows_host, int32_t W,
+             const int32_t* pairs_host, int32_t P, double compression, double eps, int32_t normalize,
+             double* scores, int32_t* index, void* stream) {
+  if (!stft || !steer || !windows_host || !scores || !index) return fail(SETK_EINVAL, "setk_ssl: null buffer");
+  if (backend < SETK_SSL_ML || backend > SETK_SSL_MUSIC) return fail(SETK_EINVAL, "setk_ssl: unknown backend %d", backend);
+  if (M < 1 || M > SETK_MAX_CHANNELS) return fail(SETK_EINVAL, "setk_ssl: M=%d outside [1, %d]", M, SETK_MAX_CHANNELS);
+  if (A < 1) return fail(SETK_EINVAL, "setk_ssl: A=%d directions", A);
+  if (B < 1 || F < 1 || T < 1 || W < 1 || B > 65535)
+    return fail(SETK_ESHAPE, "setk_ssl: bad shape B=%d F=%d T=%d W=%d", B, F, T, W);
+  if (steer_F != F) return fail(SETK_ESHAPE, "setk_ssl: steering table has %d bins, the STFT %d", steer_F, F);
+  if (N < 1 || N > SETK_SSL_MAX_MASKS || (!mask && N != 1))
+    return fail(SETK_EINVAL, "setk_ssl: N=%d masks (1..%d, 1 without a mask)", N, SETK_SSL_MAX_MASKS);
+  if (N > 1 && backend != SETK_SSL_ML) return fail(SETK_EINVAL, "setk_ssl: N=%d masks need the ML backend", N);
+  if (backend == SETK_SSL_SRP) {
+    if (!pairs_host || P < 1) return fail(SETK_EINVAL, "setk_ssl: SRP needs microphone pairs");
+    for (int p = 0; p < 2 * P; ++p)
+      if (pairs_host[p] < 0 || pairs_host[p] >= M)
+        return fail(SETK_EINVAL, "setk_ssl: pair index %d outside [0, %d)", pairs_host[p], M);
+  } else {
+    P = 0;
+  }
+  for (long long i = 0; i < (long long)B * W; ++i) {
+    const int s = windows_host[2 * i], e = windows_host[2 * i + 1];
+    if (s < 0 || e > T || s >= e)
+      return fail(SETK_EINVAL, "setk_ssl: window [%d, %d) of utterance %lld outside [0, %d] or empty", s, e,
+                  i / W, T);
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  char* ws = nullptr;
+  cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&ws), ssl_scratch_bytes(backend, B, N, M, F, T, A, W, P),
+                                  st);   // stream-ordered scratch
+  if (e != cudaSuccess) return cuda_fail(e, "setk_ssl(workspace)");
+  e = run_ssl(backend, static_cast<const float2*>(stft), B, M, F, T, static_cast<const double2*>(steer), A, mask,
+              N, windows_host, W, pairs_host, P, compression, eps, normalize, ws, scores, index, stream);
+  cudaError_t ef = cudaFreeAsync(ws, st);
+  if (e == cudaSuccess) e = ef;
+  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_ssl");
 }
 
 }  // extern "C"

@@ -23,7 +23,7 @@ DEPS[stft_spill]="common.cuh compat.cuh stft_tile.cuh fft16.cuh async_copy.cuh c
 DEPS[cov_mma]="common.cuh compat.cuh async_copy.cuh cov_spill_args.cuh mma_tf32.cuh"
 DEPS[cgmm]="common.cuh compat.cuh hermitian_solve.cuh jacobi_coop.cuh"
 DEPS[wpe]="common.cuh compat.cuh hermitian_solve.cuh"
-DEPS[spatial]="common.cuh compat.cuh"
+DEPS[spatial]="common.cuh compat.cuh ssl.cuh"
 DEPS[cm_mask]="common.cuh compat.cuh"
 pids=()
 for f in api generic weights weights_coop weights_post stft_cov_fused stft_cov_ws apply_istft_fused stft_spill cov_mma cgmm wpe spatial cm_mask; do

@@ -321,3 +321,6 @@ cudaError_t run_msc(const float2* spec, int N, int T, int F, int context, int no
 }
 
 }  // namespace setk
+
+// sound source localisation (setk_ssl): its kernels build in this translation unit
+#include "ssl.cuh"

@@ -549,3 +549,53 @@ def msc(spec, context=1, normalize=True):
         _lib.check(lib.setk_msc(_lib.ptr(spec), N, T, F, int(context), int(bool(normalize)),
                                 _lib.ptr(work), _lib.ptr(out), _lib.current_stream(spec.device)))
     return out
+
+
+# ---------------------------------------------------------------------------
+# sound source localisation on explicit STFTs (libs/ssl.py of the reference; csrc/ssl.cuh)
+# ---------------------------------------------------------------------------
+_SSL_BACKENDS = {"ml": _lib.SSL_ML, "srp": _lib.SSL_SRP, "music": _lib.SSL_MUSIC}
+
+
+def ssl(stft, steer, backend="ml", mask=None, windows=None, pairs=None, compression=0.0, eps=1e-8,
+        normalize=False):
+    """
+    DoA scores and indices, batched.  stft (B,M,F,T) complex64; steer (A,M,F) complex128;
+    mask (B,N,T,F) float32 or None; windows: (B,W,2) frame ranges [s, e) or None (one window
+    [0, T)); pairs: list of (l, r) microphone pairs (SRP).
+    Returns (scores (B,N,W,A) float64, index (B,N,W) int32), N = 1 without a mask.
+    """
+    if backend not in _SSL_BACKENDS:
+        raise ValueError(f"unknown SSL backend {backend!r}")
+    stft = _c64(stft)
+    if stft.dim() != 4:
+        raise ValueError(f"stft must be (B, M, F, T), got {tuple(stft.shape)}")
+    B, M, F, T = stft.shape
+    dev = stft.device
+    steer = torch.as_tensor(steer, device=dev).to(torch.complex128).contiguous()
+    if steer.dim() != 3 or steer.shape[1] != M:
+        raise ValueError(f"steer vector must be (A, {M}, F), got {tuple(steer.shape)}")
+    A = steer.shape[0]
+    N = 1
+    if mask is not None:
+        mask = _f32(mask, dev)
+        if mask.dim() != 4 or mask.shape[0] != B or tuple(mask.shape[2:]) != (T, F):
+            raise ValueError(f"mask must be ({B}, N, {T}, {F}), got {tuple(mask.shape)}")
+        N = mask.shape[1]
+    win = np.array([[[0, T]]] * B if windows is None else windows, dtype=np.int32).reshape(B, -1, 2)
+    win = np.ascontiguousarray(win)
+    W = win.shape[1]
+    pr = None
+    P = 0
+    if pairs is not None:
+        pr = np.ascontiguousarray(np.array(pairs, dtype=np.int32).reshape(-1, 2))
+        P = pr.shape[0]
+    scores = torch.empty((B, N, W, A), dtype=torch.float64, device=dev)
+    index = torch.empty((B, N, W), dtype=torch.int32, device=dev)
+    with _ctx(dev):
+        _lib.check(_lib.library().setk_ssl(
+            _SSL_BACKENDS[backend], _lib.ptr(stft), B, M, F, T, _lib.ptr(steer), A, steer.shape[2],
+            _lib.ptr(mask), N, ctypes.c_void_p(win.ctypes.data), W,
+            None if pr is None else ctypes.c_void_p(pr.ctypes.data), P, float(compression), float(eps),
+            int(bool(normalize)), _lib.ptr(scores), _lib.ptr(index), _lib.current_stream(dev)))
+    return scores, index
