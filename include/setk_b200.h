@@ -5,6 +5,9 @@
  *   multichannel STFT -> mask-weighted spatial covariance -> MVDR / MPDR / GEV /
  *   PMWF weight solve (+BAN, rank-1) -> beamform apply -> iSTFT (+peak norm)
  *
+ * and the front ends around it: CGMM masks, WPE / WPD, spatial features, sound
+ * source localisation and AuxIVA blind source separation.
+ *
  * Every entry point below replaces one reference interface; the citation is
  * the reference file:line (paths relative to the reference tree).  The Python
  * mirror of the reference's operator API (setk_b200/libs/{utils,stft,
@@ -356,6 +359,18 @@ int setk_ssl(int32_t backend, const void* stft, int32_t B, int32_t M, int32_t F,
              int32_t A, int32_t steer_F, const float* mask, int32_t N, const int32_t* windows_host, int32_t W,
              const int32_t* pairs_host, int32_t P, double compression, double eps, int32_t normalize,
              double* scores, int32_t* index, void* stream);
+
+/*
+ * AuxIVA: scripts/sptk/apply_auxiva.py:24-57 for every utterance of the batch.  Plan-free; scratch is
+ * stream-ordered.  fp64 after the complex64 input.
+ *   stft    c64  [B][N][F][T]   (the reference's N x T x F per utterance, bins before frames here)
+ *   out     c128 [B][N][F][T]   separated sources Y (the reference returns complex128)
+ *   status  u32 [B] or NULL     SETK_ST_SINGULAR / SETK_ST_NONFINITE (-> numpy.linalg.LinAlgError per key;
+ *                               caller zeroes it)
+ * 2 <= N <= SETK_MAX_CHANNELS, num_epochs >= 0 (0 returns X), F, T >= 1; SETK_EINVAL otherwise.
+ */
+int setk_auxiva_stft(const void* stft, int32_t B, int32_t N, int32_t F, int32_t T, int32_t num_epochs,
+                     void* out, uint32_t* status, void* stream);
 
 /* floor(y * 32768) clipped to int16: the PCM_16 conversion of
  * WaveWriter.write -> write_wav -> soundfile (data_handler.py:600-605,

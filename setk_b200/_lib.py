@@ -106,6 +106,8 @@ _PROTOTYPES = {
     "setk_ssl": (c_int, [c_int32, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_int32, c_int32,
                          c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_int32, c_double, c_double, c_int32,
                          c_void_p, c_void_p, c_void_p]),
+    "setk_auxiva_stft": (c_int, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p,
+                                 c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)

@@ -71,6 +71,8 @@ cudaError_t run_bits_to_float(const unsigned*, int, float*, void*);
 size_t ssl_scratch_bytes(int, int, int, int, int, int, int, int, int);
 cudaError_t run_ssl(int, const float2*, int, int, int, int, const double2*, int, const float*, int, const int*,
                     int, const int*, int, double, double, int, char*, double*, int*, void*);
+size_t auxiva_scratch_bytes(int, int, int, int);
+cudaError_t run_auxiva(const float2*, int, int, int, int, int, char*, double2*, unsigned*, void*);
 
 struct WeightsArgs;
 cudaError_t weights_run(int kind, double beta, int ref_channel, int rank1, int ban, const void* Rs,
@@ -707,6 +709,26 @@ int setk_ssl(int32_t backend, const void* stft, int32_t B, int32_t M, int32_t F,
   cudaError_t ef = cudaFreeAsync(ws, st);
   if (e == cudaSuccess) e = ef;
   return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_ssl");
+}
+
+// ---- AuxIVA blind source separation (auxiva.cuh, built in wpe.cu) ----
+int setk_auxiva_stft(const void* stft, int32_t B, int32_t N, int32_t F, int32_t T, int32_t num_epochs,
+                     void* out, uint32_t* status, void* stream) {
+  if (!stft || !out) return fail(SETK_EINVAL, "setk_auxiva_stft: null buffer");
+  if (N < 2 || N > SETK_MAX_CHANNELS)
+    return fail(SETK_EINVAL, "setk_auxiva_stft: N=%d outside [2, %d]", N, SETK_MAX_CHANNELS);
+  if (num_epochs < 0) return fail(SETK_EINVAL, "setk_auxiva_stft: num_epochs=%d", num_epochs);
+  if (B < 1 || F < 1 || T < 1 || B > 65535 || (long long)B * F > 2000000000LL)
+    return fail(SETK_EINVAL, "setk_auxiva_stft: bad shape B=%d F=%d T=%d", B, F, T);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  char* ws = nullptr;
+  cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&ws), auxiva_scratch_bytes(B, N, F, T), st);
+  if (e != cudaSuccess) return cuda_fail(e, "setk_auxiva_stft(workspace)");
+  e = run_auxiva(static_cast<const float2*>(stft), B, N, F, T, num_epochs, ws, static_cast<double2*>(out),
+                 status, stream);
+  cudaError_t ef = cudaFreeAsync(ws, st);
+  if (e == cudaSuccess) e = ef;
+  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_auxiva_stft");
 }
 
 }  // extern "C"

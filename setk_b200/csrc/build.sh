@@ -14,7 +14,7 @@ declare -A DEPS
 DEPS[api]="common.cuh compat.cuh"
 DEPS[generic]="common.cuh compat.cuh"
 DEPS[weights]="common.cuh compat.cuh hermitian_solve.cuh weights_args.cuh"
-DEPS[weights_coop]="common.cuh compat.cuh hermitian_solve.cuh jacobi_coop.cuh weights_args.cuh"
+DEPS[weights_coop]="common.cuh compat.cuh hermitian_solve.cuh jacobi_coop.cuh lu_coop.cuh weights_args.cuh"
 DEPS[weights_post]="common.cuh compat.cuh hermitian_solve.cuh"
 DEPS[stft_cov_fused]="common.cuh compat.cuh stft_tile.cuh fft16.cuh async_copy.cuh stft_cov_args.cuh"
 DEPS[stft_cov_ws]="common.cuh compat.cuh stft_tile.cuh fft16.cuh async_copy.cuh stft_cov_args.cuh"
@@ -22,7 +22,7 @@ DEPS[apply_istft_fused]="common.cuh compat.cuh stft_tile.cuh fft16.cuh async_cop
 DEPS[stft_spill]="common.cuh compat.cuh stft_tile.cuh fft16.cuh async_copy.cuh cov_spill_args.cuh"
 DEPS[cov_mma]="common.cuh compat.cuh async_copy.cuh cov_spill_args.cuh mma_tf32.cuh"
 DEPS[cgmm]="common.cuh compat.cuh hermitian_solve.cuh jacobi_coop.cuh"
-DEPS[wpe]="common.cuh compat.cuh hermitian_solve.cuh"
+DEPS[wpe]="common.cuh compat.cuh hermitian_solve.cuh jacobi_coop.cuh lu_coop.cuh auxiva.cuh"
 DEPS[spatial]="common.cuh compat.cuh ssl.cuh"
 DEPS[cm_mask]="common.cuh compat.cuh"
 pids=()

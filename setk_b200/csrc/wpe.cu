@@ -530,3 +530,6 @@ cudaError_t run_wpe(const float2* X, int P, int B, int C, int F, int T, int taps
 }
 
 }  // namespace setk
+
+// AuxIVA blind source separation (setk_auxiva_stft): its kernels build in this translation unit
+#include "auxiva.cuh"

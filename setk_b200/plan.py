@@ -599,3 +599,24 @@ def ssl(stft, steer, backend="ml", mask=None, windows=None, pairs=None, compress
             None if pr is None else ctypes.c_void_p(pr.ctypes.data), P, float(compression), float(eps),
             int(bool(normalize)), _lib.ptr(scores), _lib.ptr(index), _lib.current_stream(dev)))
     return scores, index
+
+
+# ---------------------------------------------------------------------------
+# AuxIVA blind source separation on explicit STFTs (apply_auxiva.py of the reference; csrc/auxiva.cuh)
+# ---------------------------------------------------------------------------
+def auxiva_from_stft(stft, num_epochs=20):
+    """
+    auxiva(X, epochs) batched (apply_auxiva.py:24-57).
+    stft (B,N,F,T) complex64 -> (separated sources (B,N,F,T) complex128, status (B,) int32).
+    """
+    stft = _c64(stft)
+    if stft.dim() != 4:
+        raise ValueError(f"stft must be (B, N, F, T), got {tuple(stft.shape)}")
+    B, N, F, T = stft.shape
+    out = torch.empty((B, N, F, T), dtype=torch.complex128, device=stft.device)
+    status = torch.zeros((B,), dtype=torch.int32, device=stft.device)
+    with _ctx(stft.device):
+        _lib.check(_lib.library().setk_auxiva_stft(
+            _lib.ptr(stft), B, N, F, T, int(num_epochs), _lib.ptr(out), _lib.ptr(status),
+            _lib.current_stream(stft.device)))
+    return out, status
