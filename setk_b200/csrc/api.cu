@@ -165,13 +165,6 @@ int setk_plan_create(const setk_config_t* cfg, setk_plan_t** plan_out) {
     win[lpad + i] = (float)w;
     wsq[lpad + i] = (float)(w * w);
   }
-  {   // windows with a constant pair sum w[n] + w[n + n_fft/2] (Hann, Hamming, rectangular, ...)
-    const int h = g.n_fft / 2;
-    const double K = (double)win[0] + (double)win[h];
-    bool ok = K > 1e-3;
-    for (int i = 0; i < h && ok; ++i) ok = fabs((double)win[i] + (double)win[i + h] - K) <= 2e-7 * K;
-    pl->win_pair_sum = ok ? (float)K : 0.f;
-  }
   cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&pl->d_window), sizeof(float) * g.n_fft);
   if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&pl->d_wsq), sizeof(float) * g.n_fft);
   if (e == cudaSuccess) e = cudaMemcpy(pl->d_window, win.data(), sizeof(float) * g.n_fft, cudaMemcpyHostToDevice);

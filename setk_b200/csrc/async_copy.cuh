@@ -60,11 +60,6 @@ __device__ inline void bulk_g2s(void* dst, const void* src, unsigned bytes, MBar
   memcpy(dst, src, bytes);
   mbar_update(b, 0, -(long long)bytes);
 }
-// L2 prefetch of a 16-byte aligned global range: no architectural effect
-__device__ inline void bulk_prefetch_l2(const void* src, unsigned bytes) {
-  if ((bytes & 15u) || (reinterpret_cast<uintptr_t>(src) & 15u))
-    emu::die("cp.async.bulk.prefetch needs a 16-byte aligned address and size");
-}
 // returns once the phase with the given parity has completed (a fresh barrier has
 // "completed" the phase of parity 1, as on the device)
 __device__ inline void mbar_wait(MBar* b, unsigned parity) {
@@ -127,10 +122,6 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, unsigned by
           smem_u32(dst)),
       "l"(src), "r"(bytes), "r"(smem_u32(b))
       : "memory");
-}
-// Asks L2 to fetch [src, src + bytes) (16-byte aligned, multiple of 16); nothing is written.
-__device__ __forceinline__ void bulk_prefetch_l2(const void* src, unsigned bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
 }
 // One try: true when the phase with the given parity has completed.  The thread may be
 // suspended by the hardware for up to `hint_ns` while it waits (it wakes when the phase

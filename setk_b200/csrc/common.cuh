@@ -89,7 +89,6 @@ struct setk_plan {
   setk::Geometry geo;
   float* d_window;       // [n_fft] analysis window, centred zero-padded, float32
   float* d_wsq;          // [n_fft] window squared (rounded from float64)
-  float win_pair_sum;    // K when window[n] + window[n + n_fft/2] == K for every n (Hann: 1), else 0
   // lazily grown workspaces (device)
   float* d_partials;     size_t partials_bytes;   // fused stft_cov partial sums
   float2* d_stft_ws;     size_t stft_ws_bytes;    // generic path STFT spill [B][C][F][T]

@@ -268,7 +268,6 @@ __global__ void __launch_bounds__(256) cov_mma_kernel(CovSpillArgs a) {
   }
 }
 
-bool cov_mma_supported(int C) { return C >= 1 && C <= 16; }
 int cov_mma_bins_per_cta(int C) { return C <= 8 ? CovMmaShape<8>::NB : CovMmaShape<16>::NB; }
 
 template <int CP>

@@ -58,34 +58,6 @@ __device__ __forceinline__ void dft16(float2 (&v)[16]) {
   for (int c = 0; c < 4; ++c) dft4(v[4 * c], v[4 * c + 1], v[4 * c + 2], v[4 * c + 3]);
 }
 
-// forward 16-point DFT of WINDOWED inputs for windows with w[n] + w[n + N/2] = 1 (Hann, after
-// scaling: every "cosine-sum" window has a constant pair sum): v[m] are the raw samples, the first
-// butterflies pair sample m with m + 8 (N/2 apart), so
-//   a w_a + c w_c = c + w_a (a - c),     a w_a - c w_c = w_a (a + c) - c        (w_c = 1 - w_a)
-// -- the same arithmetic count as multiply-then-butterfly, with HALF the window loads
-// (w8[m], m < 8, is the window of samples m).
-__device__ __forceinline__ void dft16_pairwin(float2 (&v)[16], const float2 (&w8)[8]) {
-#pragma unroll
-  for (int b = 0; b < 4; ++b) {
-    const float2 a = v[b], bb = v[4 + b], c = v[8 + b], d = v[12 + b];
-    const float2 nc = make_float2(-c.x, -c.y), nd = make_float2(-d.x, -d.y);
-    const float2 e = f2fma(w8[b], f2sub(a, c), c);            // a w_a + c w_c
-    const float2 f = f2fma(w8[b], f2add(a, c), nc);           // a w_a - c w_c
-    const float2 g = f2fma(w8[4 + b], f2sub(bb, d), d);
-    const float2 h = f2fma(w8[4 + b], f2add(bb, d), nd);
-    const float2 r = make_float2(h.y, -h.x);                  // -i h
-    v[b] = cadd(e, g);
-    v[8 + b] = csub(e, g);
-    v[4 + b] = cadd(f, r);
-    v[12 + b] = csub(f, r);
-  }
-  v[5] = mul_w16<1>(v[5]);   v[6] = mul_w16<2>(v[6]);   v[7] = mul_w16<3>(v[7]);
-  v[9] = mul_w16<2>(v[9]);   v[10] = mul_w16<4>(v[10]); v[11] = mul_w16<6>(v[11]);
-  v[13] = mul_w16<3>(v[13]); v[14] = mul_w16<6>(v[14]); v[15] = mul_w16<9>(v[15]);
-#pragma unroll
-  for (int c = 0; c < 4; ++c) dft4(v[4 * c], v[4 * c + 1], v[4 * c + 2], v[4 * c + 3]);
-}
-
 // pitch of the exchange tile in float2 units (odd -> conflict-free transposed reads)
 #define SETK_XPITCH 17
 #define SETK_ZSLOT (16 * SETK_XPITCH)   // float2 per half-warp FFT slot (272 >= 256)
@@ -167,11 +139,6 @@ __device__ __forceinline__ void halfwarp_fft256(float2 (&v)[16], float2* xch, in
 //   b: exchange through xch + second radix-16 pass
 __device__ __forceinline__ void halfwarp_fft256_a(float2 (&v)[16], const float2* tab, int lane16) {
   dft16(v);
-  twiddle_pass1_tab(v, tab, lane16);
-}
-__device__ __forceinline__ void halfwarp_fft256_a_pairwin(float2 (&v)[16], const float2 (&w8)[8],
-                                                          const float2* tab, int lane16) {
-  dft16_pairwin(v, w8);
   twiddle_pass1_tab(v, tab, lane16);
 }
 __device__ __forceinline__ void halfwarp_fft256_b(float2 (&v)[16], float2* xch, int lane16) {

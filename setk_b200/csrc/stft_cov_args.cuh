@@ -20,7 +20,6 @@ struct StftCovArgs {
   TileSched sched;       // which (utterance, tile) pairs this CTA owns
   int slots;             // partial-sum slots per utterance
   const float* window;   // [n_fft]
-  float win_pair_sum;    // K if window[n] + window[n + n_fft/2] == K for all n (Hann: 1), else 0
   float* partials;       // [B][slots][2*C*C + 2][F]
   unsigned* maxabs_bits; // [B] or null
 };

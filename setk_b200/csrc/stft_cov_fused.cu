@@ -26,7 +26,6 @@
 //   cov_finalize_kernel reduces the slots in fixed order, normalises by
 //   max(sum m, 1e-6), writes Rs, Rn c64 [B][F][C][C].
 // Algorithmic bytes per utterance: 4*C*N + 4*T*F (+4*T*F with mask_n) + 2*8*F*C^2.
-#include <cstdlib>
 #include "common.cuh"
 #include "stft_tile.cuh"
 #include "stft_cov_args.cuh"
@@ -36,18 +35,10 @@ namespace setk {
 // registers per thread of the fused kernel: 288 threads occupy 10 warp slots of the
 // register file (allocation granularity: 2 warps), so two CTAs per SM need
 // <= 65536 / (2 * 10 * 32) = 102 -> 96 registers (ncu: 112 left ONE CTA per SM)
-#ifndef SETK_SC_REGS
-#define SETK_SC_REGS 96
-#endif
-// frames per tile: 4 -> 288 threads (8 FFT warps + the Nyquist warp), 5 -> 320 threads
+constexpr int kScRegs = 96;
+// frames per tile at even C: 4 -> 288 threads (8 FFT warps + the Nyquist warp), 5 -> 320 threads
 // (10 FFT warps: the tenth warp's registers are allocated either way)
-#ifndef SETK_SC_TT
-#define SETK_SC_TT 5
-#endif
-// inter-pass FFT twiddles from a shared-memory table (1) or a register power tree (0)
-#ifndef SETK_SC_TAB
-#define SETK_SC_TAB 1
-#endif
+constexpr int kScTT = 5;
 
 // tiles before every utterance of a ragged batch (one CTA; B is small)
 __global__ void tile_prefix_kernel(const int* __restrict__ n_samples, int B, Geometry g, int TT,
@@ -85,7 +76,7 @@ cudaError_t run_tile_prefix(const int* n_samples, int B, const Geometry& g, int 
 }
 
 template <int C, int TT>
-__global__ void __maxnreg__(SETK_SC_REGS) stft_cov_kernel(StftCovArgs a) {
+__global__ void __maxnreg__(kScRegs) stft_cov_kernel(StftCovArgs a) {
   constexpr int NACC = CovAcc<C>::NACC;
   constexpr int F = kBins;
   static_assert(TT <= 8, "Nyquist lanes: one frame per lane, butterfly sum over 8 lanes");
@@ -108,14 +99,6 @@ __global__ void __maxnreg__(SETK_SC_REGS) stft_cov_kernel(StftCovArgs a) {
   for (int n = tid; n < kNfft; n += blockDim.x) sm.win[n] = 0.5f * a.window[n];
   if (tid == 0) { mbar_init(&sm.bar[0], 1); mbar_init(&sm.bar[1], 1); }
 
-  // thread constants
-#if SETK_SC_TAB
-  const float2 w1 = make_float2(1.f, 0.f);                  // unused: twiddles come from s_twtab
-#else
-  float w1s, w1c;
-  sincospif((float)(lane & 15) / 128.0f, &w1s, &w1c);      // W256^{lane16}
-  const float2 w1 = make_float2(w1c, -w1s);
-#endif
   // cov role: threads 0..255 own bins 0..255 (all frames of a tile); the Nyquist
   // bin is spread over the lanes of warp 8, one FRAME per lane, so that warp
   // issues the accumulation once per tile instead of once per frame
@@ -245,7 +228,8 @@ __global__ void __maxnreg__(SETK_SC_REGS) stft_cov_kernel(StftCovArgs a) {
         mbar_wait(&sm.bar[buf], (par >> buf) & 1u);
         par ^= 1u << buf;
       }
-      if (warp < NW) fft_tile<C, TT, SETK_SC_TAB != 0, NW>(sm, buf, nt, hop, w1, amax, s_twtab);
+      // inter-pass twiddles from s_twtab (the w1 argument is unused)
+      if (warp < NW) fft_tile<C, TT, true, NW>(sm, buf, nt, hop, make_float2(1.f, 0.f), amax, s_twtab);
       async_cur = async_next;
       cp_async_wait_all();
       __syncthreads();
@@ -321,7 +305,7 @@ __global__ void __maxnreg__(SETK_SC_REGS) stft_cov_kernel(StftCovArgs a) {
 // 16-byte stores (rows of the row-major matrix are contiguous).
 template <int C>
 __global__ void cov_finalize_kernel(const float* __restrict__ partials, int B, int F, TileSched sched,
-                                    int n_ctas, int slots, float scale, float2* __restrict__ Rs,
+                                    int n_ctas, int slots, float2* __restrict__ Rs,
                                     float2* __restrict__ Rn) {
   constexpr int NACC = CovAcc<C>::NACC;
   const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -343,8 +327,7 @@ __global__ void cov_finalize_kernel(const float* __restrict__ partials, int B, i
     for (int i = 0; i < NACC; ++i) acc[i] += pp[(long long)(which * NACC + i) * F];
     acc[NACC] += pp[(long long)(2 * NACC + which) * F];
   }
-  // scale: the spectra behind the sums were scaled by 1 / sqrt(scale) (pair-sum window path)
-  const float inv = scale / fmaxf(acc[NACC], 1e-6f);
+  const float inv = 1.0f / fmaxf(acc[NACC], 1e-6f);
   float2 M[C * C];
   int o = C;
 #pragma unroll
@@ -373,18 +356,18 @@ cudaError_t run_bits_to_float(const unsigned* bits, int n, float* out, void* str
 
 template <int C>
 static cudaError_t run_cov_finalize_t(const float* partials, int B, int F, TileSched sched, int n_ctas,
-                                      int slots, float scale, float2* Rs, float2* Rn, void* stream) {
+                                      int slots, float2* Rs, float2* Rn, void* stream) {
   const long long n = (long long)B * F;
   return launch(cov_finalize_kernel<C>, dim3((unsigned)((2 * n + 127) / 128)), dim3(128), 0, stream, true,
-                partials, B, F, sched, n_ctas, slots, scale, Rs, Rn);
+                partials, B, F, sched, n_ctas, slots, Rs, Rn);
 }
 cudaError_t run_cov_finalize(int C, const float* partials, int B, int F, TileSched sched, int n_ctas,
-                             int slots, float scale, float2* Rs, float2* Rn, void* stream) {
+                             int slots, float2* Rs, float2* Rn, void* stream) {
   switch (C) {
-    case 1: return run_cov_finalize_t<1>(partials, B, F, sched, n_ctas, slots, scale, Rs, Rn, stream);
-    case 2: return run_cov_finalize_t<2>(partials, B, F, sched, n_ctas, slots, scale, Rs, Rn, stream);
-    case 3: return run_cov_finalize_t<3>(partials, B, F, sched, n_ctas, slots, scale, Rs, Rn, stream);
-    case 4: return run_cov_finalize_t<4>(partials, B, F, sched, n_ctas, slots, scale, Rs, Rn, stream);
+    case 1: return run_cov_finalize_t<1>(partials, B, F, sched, n_ctas, slots, Rs, Rn, stream);
+    case 2: return run_cov_finalize_t<2>(partials, B, F, sched, n_ctas, slots, Rs, Rn, stream);
+    case 3: return run_cov_finalize_t<3>(partials, B, F, sched, n_ctas, slots, Rs, Rn, stream);
+    case 4: return run_cov_finalize_t<4>(partials, B, F, sched, n_ctas, slots, Rs, Rn, stream);
     default: return cudaErrorInvalidValue;
   }
 }
@@ -403,7 +386,7 @@ static cudaError_t run_stft_cov_t(setk_plan* pl, StftCovArgs a, int B, int n_cta
   if (e != cudaSuccess) return e;
   e = launch(stft_cov_kernel<C, TT>, dim3(n_ctas), dim3(TT > 4 ? 320 : 288), smem, stream, false, a);
   if (e != cudaSuccess) return e;
-  e = run_cov_finalize_t<C>(a.partials, B, a.g.F, a.sched, n_ctas, a.slots, 1.0f, Rs, Rn, stream);
+  e = run_cov_finalize_t<C>(a.partials, B, a.g.F, a.sched, n_ctas, a.slots, Rs, Rn, stream);
   if (e != cudaSuccess) return e;
   if (maxabs) e = run_bits_to_float(a.maxabs_bits, B, maxabs, stream);
   return e;
@@ -441,11 +424,7 @@ int stft_cov_pick_chunks(const setk_plan* pl, int B, int T) {
 }
 
 // CTA slots of the fused kernels (2 CTAs per SM resident: registers and shared memory)
-int fused_cta_slots(const setk_plan* pl) {
-  static const char* env = getenv("SETK_FUSED_CTAS_PER_SM");   // measurement knob
-  const int per_sm = env && atoi(env) > 0 ? atoi(env) : 2;
-  return per_sm * pl->sm_count;
-}
+int fused_cta_slots(const setk_plan* pl) { return 2 * pl->sm_count; }
 
 // launch shape of the persistent schedule for a batch of B utterances of <= T frames
 void fused_schedule(const setk_plan* pl, int B, int T, int TT, int* n_ctas, int* slots, int* min_quota) {
@@ -456,9 +435,10 @@ void fused_schedule(const setk_plan* pl, int B, int T, int TT, int* n_ctas, int*
   *n_ctas = sched_grid(B * tiles_max, G, *min_quota);
 }
 
-// frames per tile of the instantiation that serves C channels (an odd C with TT = 5
-// would leave an odd number of half-warp jobs)
-static int sc_tt(int C) { return (C % 2 == 0) ? SETK_SC_TT : 4; }
+// frames per tile of the instantiation that serves C <= 3 channels (an odd C with TT = 5
+// would leave an odd number of half-warp jobs); the warp-specialised build for C = 4 also
+// uses 4 (stft_cov_ws_tt)
+static int sc_tt(int C) { return C == 2 ? kScTT : 4; }
 
 size_t stft_cov_partial_bytes(const setk_plan* pl, int B, int T) {
   int n_ctas, slots, mq;
@@ -470,19 +450,12 @@ bool stft_cov_ws_supported(const Geometry& g);
 cudaError_t run_stft_cov_ws(setk_plan*, const float*, const int*, int, int, int, const float*, const float*,
                             unsigned, int*, float*, unsigned*, float2*, float2*, float*, void*);
 
-// which build of the fused kernel serves this geometry: the warp-specialised one
-// (stft_cov_ws.cu) where it exists, unless SETK_SC_IMPL=classic (measurement knob)
-static bool use_ws(const Geometry& g) {
-  const char* env = getenv("SETK_SC_IMPL");
-  if (env && env[0] == 'c') return false;
-  return stft_cov_ws_supported(g);
-}
-
 cudaError_t run_stft_cov_fused(setk_plan* pl, const float* audio, const int* n_samples, int B, int N,
                                int T, const float* mask_s, const float* mask_n, unsigned flags,
                                int* tile_prefix, float* partials, unsigned* maxabs_bits, float2* Rs,
                                float2* Rn, float* maxabs, void* stream) {
-  if (use_ws(pl->geo))
+  // C = 4: the warp-specialised build (stft_cov_ws.cu)
+  if (stft_cov_ws_supported(pl->geo))
     return run_stft_cov_ws(pl, audio, n_samples, B, N, T, mask_s, mask_n, flags, tile_prefix, partials,
                            maxabs_bits, Rs, Rn, maxabs, stream);
   const int TT = sc_tt(pl->geo.C);
@@ -502,14 +475,12 @@ cudaError_t run_stft_cov_fused(setk_plan* pl, const float* audio, const int* n_s
     a.sched.prefix = tile_prefix;
   }
   a.window = pl->d_window;
-  a.win_pair_sum = 0.f;
   a.partials = partials;
   a.maxabs_bits = maxabs_bits;
   switch (pl->geo.C) {
     case 1: return run_stft_cov_t<1, 4>(pl, a, B, n_ctas, Rs, Rn, maxabs, stream);
-    case 2: return run_stft_cov_t<2, SETK_SC_TT>(pl, a, B, n_ctas, Rs, Rn, maxabs, stream);
+    case 2: return run_stft_cov_t<2, kScTT>(pl, a, B, n_ctas, Rs, Rn, maxabs, stream);
     case 3: return run_stft_cov_t<3, 4>(pl, a, B, n_ctas, Rs, Rn, maxabs, stream);
-    case 4: return run_stft_cov_t<4, SETK_SC_TT>(pl, a, B, n_ctas, Rs, Rn, maxabs, stream);
     default: return cudaErrorInvalidValue;
   }
 }

@@ -39,8 +39,6 @@
 //   cov_finalize_kernel exactly as before (deterministic, no float atomics).
 //
 // Algorithmic bytes per utterance: 4*C*N + 4*T*F (+4*T*F with mask_n) + 2*8*F*C^2.
-#include <cstdlib>
-#include <cstring>
 #include "common.cuh"
 #include "stft_tile.cuh"
 #include "stft_cov_args.cuh"
@@ -49,22 +47,8 @@ namespace setk {
 
 // Register budgets.  The CTA's pool is what it was launched with (80 x 384 = 30 720, two
 // CTAs per SM); after the re-budgeting 8 x 32 x 64 + 4 x 32 x 112 = 30 720 exactly.
-#ifndef SETK_WS_FFT_REGS
-#define SETK_WS_FFT_REGS 64
-#endif
-#ifndef SETK_WS_COV_REGS
-#define SETK_WS_COV_REGS 112
-#endif
+constexpr int kWsFftRegs = 64, kWsCovRegs = 112;
 #define SETK_WS_LAUNCH_REGS 80
-// measurement knob: 1 puts the covariance warps at the LOW warp ids (first hardware pass)
-#ifndef SETK_WS_COV_FIRST
-#define SETK_WS_COV_FIRST 0
-#endif
-
-enum { WS_MODE_TMA = 0, WS_MODE_PAIRWIN = 1, WS_MODE_DIRECT = 2 };
-#ifndef SETK_WS_L2_PREFETCH
-#define SETK_WS_L2_PREFETCH 1
-#endif
 constexpr int kWsCovThreads = 128, kWsFftThreads = 256, kWsThreads = 384;
 constexpr int kWsBarFft = 1, kWsBarCov = 2;   // named barriers (0 is __syncthreads)
 #ifndef SETK_TABLE_CHUNK
@@ -215,13 +199,12 @@ __device__ __forceinline__ void ws_stage_scalar(const WsSmem<C>& sm, const float
 // ---------------------------------------------------------------------------
 // FFT role: threads 0..255, half-warp job = thread / 16 = frame * C + channel
 // ---------------------------------------------------------------------------
-template <int C, bool HAS_MN, int MODE>
+template <int C, bool HAS_MN>
 __device__ __forceinline__ void ws_fft_role(const StftCovArgs& a, const WsSmem<C>& sm, int lo, int hi, int q,
                                             bool vec_ok) {
   constexpr int TT = WsShape<C>::TT;
   constexpr int NR = HAS_MN ? 2 : 1, MS = HAS_MN ? 2 : 3;
-  constexpr bool PAIRWIN = MODE == WS_MODE_PAIRWIN, DIRECT = MODE == WS_MODE_DIRECT;
-  const int ftid = (int)threadIdx.x - (SETK_WS_COV_FIRST ? kWsCovThreads : 0);
+  const int ftid = (int)threadIdx.x;
   const int lane = ftid & 31, lane16 = lane & 15;
   const int fwarp = ftid >> 5;
   const int half = lane >> 4;
@@ -250,13 +233,7 @@ __device__ __forceinline__ void ws_fft_role(const StftCovArgs& a, const WsSmem<C
     if (nt <= 0) return false;
     const float* xb = a.audio + (long long)d.b * C * a.N;
     if (d.flags & WS_AUDIO_BULK) {
-      if (DIRECT) {       // the FFT threads will read the samples themselves: warm L2 a tile ahead
-        if (SETK_WS_L2_PREFETCH && ftid < C)
-          bulk_prefetch_l2(xb + (long long)ftid * a.N + d.t0 * hop - pad,
-                           (unsigned)(((nt - 1) * hop + kNfft) * sizeof(float)));
-      } else if (ftid == 0) {
-        ws_stage_bulk<C>(sm, xb, a.N, d.t0, nt, hop, pad);
-      }
+      if (ftid == 0) ws_stage_bulk<C>(sm, xb, a.N, d.t0, nt, hop, pad);
       return false;
     }
     ws_stage_scalar<C>(sm, xb, a.N, d.nb, d.t0, nt, hop, pad, ftid);
@@ -278,49 +255,30 @@ __device__ __forceinline__ void ws_fft_role(const StftCovArgs& a, const WsSmem<C
       const WsTile d = sm.tiles[i];
       const int nt = (int)(d.flags & WS_NT);
       float2 v[16];
-      float2 w8[8];                                  // PAIRWIN: window of the first half frame
-      const bool from_global = DIRECT && (d.flags & WS_AUDIO_BULK);
       if (nt > 0) {
-        if (!DIRECT && (d.flags & WS_AUDIO_BULK)) { mbar_wait(sm.bar_audio, apar); apar ^= 1u; }
+        if (d.flags & WS_AUDIO_BULK) { mbar_wait(sm.bar_audio, apar); apar ^= 1u; }
         // a dead frame (fr >= nt, only in an utterance's last tile) re-transforms the last live
         // one: its spectrum is never read and max|x| sees nothing new
         const int fr_src = imin(fr, nt - 1);
         // max|x|: with hop = n_fft / 2 the first halves of the frames tile the signal, so only an
         // utterance's last frame looks at its second half as well
         const bool amax_full = hop != kM || ((d.flags & WS_UTT_END) && fr >= nt - 1);
-        // DIRECT: an interior tile's samples come straight from global memory (a half-warp reads
-        // 128 contiguous bytes per load, each sample twice across the 50 % frame overlap: L1/L2
-        // hits) and never cross shared memory; edge tiles keep the staged path
-        const float* src = from_global
-            ? a.audio + ((long long)d.b * C + ch) * a.N + ((d.t0 + fr_src) * hop - pad) + 2 * lane16
-            : sm.audio + ch * sm.Lp + fr_src * hop + 2 * lane16;
+        const float* src = sm.audio + ch * sm.Lp + fr_src * hop + 2 * lane16;
         const float* wsrc = sm.win + 2 * lane16;
-        if (from_global) {
 #pragma unroll
-          for (int m1 = 0; m1 < 16; ++m1) v[m1] = __ldg(reinterpret_cast<const float2*>(src + 32 * m1));
-        } else {
-#pragma unroll
-          for (int m1 = 0; m1 < 16; ++m1) v[m1] = *reinterpret_cast<const float2*>(src + 32 * m1);
-        }
+        for (int m1 = 0; m1 < 16; ++m1) v[m1] = *reinterpret_cast<const float2*>(src + 32 * m1);
 #pragma unroll
         for (int m1 = 0; m1 < 16; ++m1) {
           if (m1 < 8 || amax_full) amax = fmaxf(amax, fmaxf(fabsf(v[m1].x), fabsf(v[m1].y)));
-          if (PAIRWIN) {                             // the window rides in the first butterflies
-            if (m1 < 8) w8[m1] = *reinterpret_cast<const float2*>(wsrc + 32 * m1);
-          } else {
-            v[m1] = f2mul(v[m1], *reinterpret_cast<const float2*>(wsrc + 32 * m1));
-          }
+          v[m1] = f2mul(v[m1], *reinterpret_cast<const float2*>(wsrc + 32 * m1));
         }
       }
       // every FFT warp holds its samples: the staging buffer is free
-      if (!from_global) named_bar_sync(kWsBarFft, kWsFftThreads);
+      named_bar_sync(kWsBarFft, kWsFftThreads);
       const bool has_next = c0 + i + 1 < hi;
       bool scalar_next = false;
       if (has_next) scalar_next = stage(sm.tiles[i + 1]);
-      if (nt > 0) {
-        if (PAIRWIN) halfwarp_fft256_a_pairwin(v, w8, sm.twtab, lane16);
-        else halfwarp_fft256_a(v, sm.twtab, lane16);
-      }
+      if (nt > 0) halfwarp_fft256_a(v, sm.twtab, lane16);
       const int s = n & 1;
       mbar_wait(&sm.z_empty[s], ((unsigned)(n >> 1) & 1u) ^ 1u);
       // the covariance warps are done with tile n - 2: its Z slot, and the mask slot tile n + 1
@@ -455,7 +413,7 @@ __device__ __forceinline__ void ws_cov_role(const StftCovArgs& a, const WsSmem<C
   constexpr int TT = WsShape<C>::TT, NPAIR = WsShape<C>::NPAIR, NACC = WsShape<C>::NACC;
   constexpr int ROWS128 = WsShape<C>::ROWS128, F = kBins;
   constexpr int NR = HAS_MN ? 2 : 1, MS = HAS_MN ? 2 : 3;
-  const int tid = (int)threadIdx.x - (SETK_WS_COV_FIRST ? 0 : kWsFftThreads), lane = tid & 31, warp = tid >> 5;
+  const int tid = (int)threadIdx.x - kWsFftThreads, lane = tid & 31, warp = tid >> 5;
   const int bk = tid, bm = kM - tid;                       // the pair's bins
   const int zk = tid, zn = (kM - tid) & (kM - 1);          // their half-size spectrum entries
   const float2 tw = split_twiddle(tid);
@@ -538,12 +496,8 @@ __device__ __forceinline__ void ws_cov_role(const StftCovArgs& a, const WsSmem<C
   }
 }
 
-// PAIRWIN: the window has a constant pair sum K = w[n] + w[n + 256] (Hann: 1): the FFT warps load
-// half the window (scaled by 1 / K) and fold it into the first butterflies; the spectra come out
-// scaled by 2 / K, which cov_finalize_kernel takes back (K^2 / 4 on the sums).
-template <int C, bool HAS_MN, int MODE>
+template <int C, bool HAS_MN>
 __global__ void __maxnreg__(SETK_WS_LAUNCH_REGS) stft_cov_ws_kernel(StftCovArgs a) {
-  constexpr bool PAIRWIN = MODE == WS_MODE_PAIRWIN;
   SETK_DYN_SMEM(float, smem);
   WsSmem<C> sm;
   sm.carve(smem, a.g.hop, HAS_MN ? 2 : 1);
@@ -557,7 +511,7 @@ __global__ void __maxnreg__(SETK_WS_LAUNCH_REGS) stft_cov_ws_kernel(StftCovArgs 
   if (lo >= hi) return;
 
   for (int n = tid; n < kNfft; n += kWsThreads)
-    sm.win[n] = PAIRWIN ? a.window[n] / a.win_pair_sum : 0.5f * a.window[n];
+    sm.win[n] = 0.5f * a.window[n];
   twiddle_table_fill(sm.twtab, tid, kWsThreads);
   if (tid == 0) {
     mbar_init(sm.bar_audio, 1);
@@ -569,12 +523,12 @@ __global__ void __maxnreg__(SETK_WS_LAUNCH_REGS) stft_cov_ws_kernel(StftCovArgs 
   __syncthreads();
   const bool vec_ok = ((a.N & 3) == 0) && ((a.g.hop & 3) == 0) && ((a.g.pad & 3) == 0) &&
                       ((reinterpret_cast<uintptr_t>(a.audio) & 15) == 0);
-  if (SETK_WS_COV_FIRST ? tid < kWsCovThreads : tid >= kWsFftThreads) {
-    setmaxnreg_inc<SETK_WS_COV_REGS>();
+  if (tid >= kWsFftThreads) {
+    setmaxnreg_inc<kWsCovRegs>();
     ws_cov_role<C, HAS_MN>(a, sm, lo, hi, q, vec_ok);
   } else {
-    setmaxnreg_dec<SETK_WS_FFT_REGS>();
-    ws_fft_role<C, HAS_MN, MODE>(a, sm, lo, hi, q, vec_ok);
+    setmaxnreg_dec<kWsFftRegs>();
+    ws_fft_role<C, HAS_MN>(a, sm, lo, hi, q, vec_ok);
   }
 }
 
@@ -583,7 +537,7 @@ cudaError_t run_bits_to_float(const unsigned* bits, int n, float* out, void* str
 cudaError_t run_tile_prefix(const int* n_samples, int B, const Geometry& g, int TT, int T_cap,
                             int* prefix, void* stream);
 cudaError_t run_cov_finalize(int C, const float* partials, int B, int F, TileSched sched, int n_ctas,
-                             int slots, float scale, float2* Rs, float2* Rn, void* stream);
+                             int slots, float2* Rs, float2* Rn, void* stream);
 void fused_schedule(const setk_plan* pl, int B, int T, int TT, int* n_ctas, int* slots, int* min_quota);
 
 bool stft_cov_ws_supported(const Geometry& g) {
@@ -593,18 +547,16 @@ bool stft_cov_ws_supported(const Geometry& g) {
 }
 int stft_cov_ws_tt(int C) { return 16 / C; }
 
-template <int C, bool HAS_MN, int MODE>
+template <int C, bool HAS_MN>
 static cudaError_t run_ws_t(StftCovArgs a, int B, int n_ctas, float2* Rs, float2* Rn, float* maxabs,
                             void* stream) {
   const size_t smem = WsSmem<C>::bytes(a.g.hop, HAS_MN ? 2 : 1);
-  cudaError_t e = cudaFuncSetAttribute(stft_cov_ws_kernel<C, HAS_MN, MODE>,
+  cudaError_t e = cudaFuncSetAttribute(stft_cov_ws_kernel<C, HAS_MN>,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  e = launch(stft_cov_ws_kernel<C, HAS_MN, MODE>, dim3(n_ctas), dim3(kWsThreads), smem, stream, false,
-             a);
+  e = launch(stft_cov_ws_kernel<C, HAS_MN>, dim3(n_ctas), dim3(kWsThreads), smem, stream, false, a);
   if (e != cudaSuccess) return e;
-  const float scale = MODE == WS_MODE_PAIRWIN ? 0.25f * a.win_pair_sum * a.win_pair_sum : 1.0f;
-  e = run_cov_finalize(C, a.partials, B, a.g.F, a.sched, n_ctas, a.slots, scale, Rs, Rn, stream);
+  e = run_cov_finalize(C, a.partials, B, a.g.F, a.sched, n_ctas, a.slots, Rs, Rn, stream);
   if (e != cudaSuccess) return e;
   if (maxabs) e = run_bits_to_float(a.maxabs_bits, B, maxabs, stream);
   return e;
@@ -631,25 +583,11 @@ cudaError_t run_stft_cov_ws(setk_plan* pl, const float* audio, const int* n_samp
     a.sched.prefix = tile_prefix;
   }
   a.window = pl->d_window;
-  // SETK_WS_PAIRWIN=1 (measurement knob): window folded into the first butterflies.  Not the
-  // default: the eight window pairs it keeps in registers push the 64-register FFT warps into spills.
-  const char* env_pw = getenv("SETK_WS_PAIRWIN");
-  a.win_pair_sum = (env_pw && env_pw[0] == '1') ? pl->win_pair_sum : 0.f;
   a.partials = partials;
   a.maxabs_bits = maxabs_bits;
-  const bool pw = a.win_pair_sum > 0.f;
-  // SETK_WS_AUDIO=direct (measurement knob): interior tiles' samples by LDG instead of TMA staging
-  const char* env_au = getenv("SETK_WS_AUDIO");
-  const bool direct = !pw && env_au && strcmp(env_au, "direct") == 0;
   if (pl->geo.C != 4) return cudaErrorInvalidValue;
-  if (mask_n) {
-    if (pw) return run_ws_t<4, true, WS_MODE_PAIRWIN>(a, B, n_ctas, Rs, Rn, maxabs, stream);
-    if (direct) return run_ws_t<4, true, WS_MODE_DIRECT>(a, B, n_ctas, Rs, Rn, maxabs, stream);
-    return run_ws_t<4, true, WS_MODE_TMA>(a, B, n_ctas, Rs, Rn, maxabs, stream);
-  }
-  if (pw) return run_ws_t<4, false, WS_MODE_PAIRWIN>(a, B, n_ctas, Rs, Rn, maxabs, stream);
-  if (direct) return run_ws_t<4, false, WS_MODE_DIRECT>(a, B, n_ctas, Rs, Rn, maxabs, stream);
-  return run_ws_t<4, false, WS_MODE_TMA>(a, B, n_ctas, Rs, Rn, maxabs, stream);
+  if (mask_n) return run_ws_t<4, true>(a, B, n_ctas, Rs, Rn, maxabs, stream);
+  return run_ws_t<4, false>(a, B, n_ctas, Rs, Rn, maxabs, stream);
 }
 
 }  // namespace setk

@@ -525,17 +525,12 @@ cudaError_t run_stft_spill(setk_plan* pl, const float* audio, const int* n_sampl
 }
 
 int stft_cov_pick_chunks(const setk_plan*, int, int);
-bool cov_mma_supported(int C);
 int cov_mma_bins_per_cta(int C);
 cudaError_t run_cov_mma(const CovSpillArgs& a, int B, void* stream);
 
 // C >= 5: the covariance is a real dense contraction (2C x 2C Gram blocks over T frames) and runs
-// on the tensor cores (cov_mma.cu) unless SETK_COV_IMPL=cuda (measurement knob)
-static bool use_cov_mma(int C) {
-  const char* env = getenv("SETK_COV_IMPL");
-  if (env && env[0] == 'c') return false;
-  return C >= 5 && cov_mma_supported(C);
-}
+// on the tensor cores (cov_mma.cu); C <= 4 keeps the CUDA-core cov_spill_kernel
+static bool use_cov_mma(int C) { return C >= 5; }
 
 // chunks of frames per utterance for the covariance pass over the workspace
 int cov_spill_chunks(const setk_plan* pl, int B, int T) {
@@ -557,10 +552,13 @@ int cov_spill_chunks(const setk_plan* pl, int B, int T) {
 
 template <int C>
 static cudaError_t run_cov_spill_t(const CovSpillArgs& a, int B, float2* Rs, float2* Rn, void* stream) {
-  const int nbb = (a.F + 287) / 288;
-  cudaError_t e = use_cov_mma(C) ? run_cov_mma(a, B, stream)
-                                 : launch(cov_spill_kernel<C>, dim3(a.n_chunks * nbb, C, B), dim3(288), 0,
-                                          stream, true, a);
+  cudaError_t e;
+  if constexpr (C >= 5) {
+    e = run_cov_mma(a, B, stream);
+  } else {
+    const int nbb = (a.F + 287) / 288;
+    e = launch(cov_spill_kernel<C>, dim3(a.n_chunks * nbb, C, B), dim3(288), 0, stream, true, a);
+  }
   if (e != cudaSuccess) return e;
   const long long n = (long long)B * a.F * C;
   return launch(cov_spill_finalize_kernel<C>, dim3((unsigned)((n + 127) / 128)), dim3(128), 0, stream,

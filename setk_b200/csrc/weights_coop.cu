@@ -10,8 +10,6 @@
 //
 // Kinds: MVDR (beamformer.py:527-539), MPDR (555-573), GEVD / PEVD (31-63, 674-682), with BAN
 // (14-28).  MPDR-whiten, PMWF and the rank-1 options stay on weights.cu.
-#include <cstdlib>
-#include <cstring>
 #include "jacobi_coop.cuh"
 #include "lu_coop.cuh"
 #include "weights_args.cuh"
@@ -259,10 +257,7 @@ bool weights_coop_supported(const WeightsArgs& a, int C) {
     // C = 4: four threads per bin for the eigenvector kinds (the one-thread solve is a single long fp64
     // dependency chain per bin that fills few warp slots); the Cholesky kinds and C < 4 keep the
     // register-resident one-thread solve.
-    // SETK_W_IMPL=thread / coop (measurement knob, read per call) forces either.
-    const char* env = getenv("SETK_W_IMPL");
-    if (C != 4 || (env && strcmp(env, "thread") == 0)) return false;
-    if (!coop_two_matrices(a) && !(env && strcmp(env, "coop") == 0)) return false;
+    if (C != 4 || !coop_two_matrices(a)) return false;
   }
   if (a.rank1 != SETK_RANK1_NONE) return false;
   return a.kind == SETK_BF_MVDR || a.kind == SETK_BF_MPDR || a.kind == SETK_BF_GEVD ||

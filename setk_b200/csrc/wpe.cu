@@ -21,7 +21,6 @@
 // All arithmetic is fp64 (the reference computes in the dtype of its input,
 // complex64; see oracle/wpe_oracle.py).
 #include <cstdlib>
-#include <cstring>
 #include "common.cuh"
 #include "hermitian_solve.cuh"
 
@@ -198,155 +197,6 @@ __global__ void __launch_bounds__(512) wpe_corr_kernel(WpeArgs a) {
     }
 }
 
-// ---------------------------------------------------------------------------
-// The same correlation on the fp64 TENSOR CORES (mma.sync.m8n8k4.f64, SASS DMMA): SURVEY.md
-// section 8f-2 -- R = Y~ diag(1/lambda) Y~^H is the one real dense contraction of the repository
-// (NK x (NK + C) = 60 x 66 complex outputs over T = 626 frames per bin).
-// A 4 x 4 COMPLEX tile of [R | r] is one 8 x 8 real tile: rows (Re y_i, i = 4I..4I+3 | Im y_i),
-// columns interleaved (Re a_j, Im a_j), K = 4 frames per instruction:
-//   lane (g, q): A element = part (g >> 2) of row 4I + (g & 3) at frame q, times 1 / lambda
-//                B element = part (g & 1) of column 4J + (g >> 1) at frame q
-//                D elements = (row g, columns Re / Im of column 4J + q)
-//   R_ij = (ReRe + ImIm) + i (ImRe - ReIm): lanes g and g ^ 4 exchange once per bin (epilogue).
-// A warp owns blocks of 2 x 4 tiles (S blocks, 16 S accumulator doubles per lane): 6 operand loads
-// per 8 DMMA.  Only tiles with J >= I are computed (upper block triangle), like the DFMA kernel.
-// ---------------------------------------------------------------------------
-#ifdef SETK_EMU
-__device__ inline void dmma_8x8x4(double (&d)[2], double a, double b) {
-  double mine[2] = {a, b}, all[2 * 32];
-  emu::warp_allgather64(mine, 2, all);
-  const int lane = emu::g_tid & 31, g = lane >> 2, q = lane & 3;
-  for (int e = 0; e < 2; ++e) {
-    double s = d[e];
-    for (int k = 0; k < 4; ++k) s += all[g * 4 + k] * all[32 + (2 * q + e) * 4 + k];   // A[g][k] B[k][2q+e]
-    d[e] = s;
-  }
-}
-#else
-__device__ __forceinline__ void dmma_8x8x4(double (&d)[2], double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-               : "+d"(d[0]), "+d"(d[1]) : "d"(a), "d"(b));
-}
-#endif
-
-// blocks of 2 x 4 tiles that touch the upper block triangle, in row-major order
-SETK_HD inline int wpe_dmma_blocks(int NK, int NA) {
-  const int RT = (NK + 3) / 4, CT = (NA + 3) / 4;
-  int n = 0;
-  for (int bi = 0; 2 * bi < RT; ++bi)
-    for (int bj = 0; 4 * bj < CT; ++bj)
-      if (4 * bj + 3 >= 2 * bi) ++n;
-  return n;
-}
-
-template <int S>
-__global__ void __launch_bounds__(512) wpe_corr_dmma_kernel(WpeArgs a) {
-  SETK_DYN_SMEM(double, sm);
-  cd* xs; double* linv; double* L; cd* Gs;
-  wpe_carve(sm, a, xs, linv, L, Gs);
-  const int bin = blockIdx.x, b = bin / a.F, f = bin - b * a.F;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
-  const int g = lane >> 2, q = lane & 3;
-  const int hist = a.taps + a.delay, C = a.C, NK = a.NK, NA = NK + C;
-  const int RT = (NK + 3) / 4, CT = (NA + 3) / 4;
-  if (a.use_filter)
-    for (int e = tid; e < NK * C; e += blockDim.x) {
-      const double* gp = a.G + ((long long)bin * NK * C + e) * 2;
-      Gs[e] = cd_make(gp[0], gp[1]);
-    }
-  // this warp's blocks: the e-th needed block goes to warp e % nw, slot e / nw
-  int bI[S], bJ[S];          // first row tile / first column tile of the slot's block (-1: unused)
-  constexpr int kNone = -(1 << 30);   // "no operand" (real offsets may be negative: the delayed rows)
-  int offA[S][2], offB[S][4];  // double index (relative to frame t0's position) of this lane's operand
-#pragma unroll
-  for (int s = 0; s < S; ++s) { bI[s] = -1; bJ[s] = -1; }
-  {
-    int e = 0;
-    for (int bi = 0; 2 * bi < RT; ++bi)
-      for (int bj = 0; 4 * bj < CT; ++bj)
-        if (4 * bj + 3 >= 2 * bi) {
-          if (e % nw == warp) {
-#pragma unroll
-            for (int s = 0; s < S; ++s)
-              if (s == e / nw) { bI[s] = 2 * bi; bJ[s] = 4 * bj; }
-          }
-          ++e;
-        }
-  }
-#pragma unroll
-  for (int s = 0; s < S; ++s) {
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      const int m = 4 * (bI[s] + r) + (g & 3);
-      offA[s][r] = (bI[s] >= 0 && m < NK) ? 2 * ((m % C) * a.Wp - (m / C) - a.delay) + (g >> 2) : kNone;
-    }
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      const int j = 4 * (bJ[s] + c) + (g >> 1);
-      int o = kNone;
-      if (bJ[s] >= 0 && j < NK) o = 2 * ((j % C) * a.Wp - (j / C) - a.delay) + (g & 1);
-      else if (bJ[s] >= 0 && j < NA) o = 2 * ((j - NK) * a.Wp) + (g & 1);
-      offB[s][c] = o;
-    }
-  }
-  double acc[S][2][4][2];
-#pragma unroll
-  for (int s = 0; s < S; ++s)
-#pragma unroll
-    for (int r = 0; r < 2; ++r)
-#pragma unroll
-      for (int c = 0; c < 4; ++c) { acc[s][r][c][0] = 0.0; acc[s][r][c][1] = 0.0; }
-
-  for (int t0 = 0; t0 < a.T; t0 += a.Tc) {
-    const int n = imin(a.Tc, a.T - t0);
-    wpe_chunk_prologue(a, b, f, t0, n, xs, linv, L, Gs);
-    const double* xt = reinterpret_cast<const double*>(xs + a.ctx + hist);   // frame t0, as doubles
-    for (int u = 0; u < n; u += 4) {
-      const bool live = u + q < n;
-      const double w = live ? linv[u + q] : 0.0;
-      const int fo = 2 * (u + q);
-#pragma unroll
-      for (int s = 0; s < S; ++s) {
-        if (bI[s] < 0) continue;                               // warp-uniform
-        double av[2], bv[4];
-#pragma unroll
-        for (int r = 0; r < 2; ++r) av[r] = (offA[s][r] != kNone && live) ? xt[offA[s][r] + fo] * w : 0.0;
-#pragma unroll
-        for (int c = 0; c < 4; ++c) bv[c] = (offB[s][c] != kNone && live) ? xt[offB[s][c] + fo] : 0.0;
-#pragma unroll
-        for (int r = 0; r < 2; ++r)
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            const int I = bI[s] + r, J = bJ[s] + c;
-            if (I < RT && J < CT && J >= I) dmma_8x8x4(acc[s][r][c], av[r], bv[c]);   // warp-uniform
-          }
-      }
-    }
-  }
-  // ---- epilogue: lanes g and g ^ 4 hold the Re-row and the Im-row sums of the same (i, j) ----
-  double* R = a.Raug + (long long)bin * NK * NA * 2;
-#pragma unroll
-  for (int s = 0; s < S; ++s) {
-    if (bI[s] < 0) continue;
-#pragma unroll
-    for (int r = 0; r < 2; ++r)
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        const int I = bI[s] + r, J = bJ[s] + c;
-        if (!(I < RT && J < CT && J >= I)) continue;
-        const double c0 = acc[s][r][c][0], c1 = acc[s][r][c][1];
-        const double p1 = __shfl_xor_sync(0xffffffffu, c1, 16);
-        const int i = 4 * I + (g & 3), j = 4 * J + q;
-        const bool imag = (g >> 2) != 0;
-        const double v = imag ? c0 - p1 : c0 + p1;             // Im R_ij : Re R_ij
-        if (i < NK && j < NA && j >= i) {
-          R[((long long)i * NA + j) * 2 + (imag ? 1 : 0)] = v;
-          if (j > i && j < NK) R[((long long)j * NA + i) * 2 + (imag ? 1 : 0)] = imag ? -v : v;
-        }
-      }
-  }
-}
-
 // CTA per bin; thread (r, cg) = (tid / 4, tid % 4) owns columns j = cg (mod 4) of row r of
 // the augmented [R | r].  The multipliers are used and dropped (the right-hand sides
 // ride along), so a step costs three barriers: pivot vote, row swap, elimination.
@@ -467,7 +317,7 @@ cudaError_t run_wpe(const float2* X, int P, int B, int C, int F, int T, int taps
   a.NK = C * taps;
   a.Tc = wpe_chunk_frames(C, T, taps, delay, ctx);
   if (const char* env = getenv("SETK_WPE_CHUNK")) {     // test knob: force chunking of short inputs
-    const int v = (atoi(env) + 3) & ~3;                   // whole 4-frame tensor-core steps
+    const int v = (atoi(env) + 3) & ~3;                   // a multiple of 4 frames
     if (v >= 4 && v < a.Tc) a.Tc = v;
   }
   a.Wp = a.Tc + 2 * ctx + taps + delay;
@@ -479,31 +329,10 @@ cudaError_t run_wpe(const float2* X, int P, int B, int C, int F, int T, int taps
   const int NA = a.NK + C, RT = (a.NK + 3) / 4, CT = (NA + 3) / 4;
   const int ntiles = RT * CT - RT * (RT - 1) / 2;
   const int corr_threads = ((ntiles + 31) / 32) * 32;
-  // tensor-core correlation: <= 16 warps, <= 3 blocks of 2 x 4 tiles per warp.  On an H100 SXM at
-  // 700 W (6 ch x 10 taps, B = 64, 3 iterations) the whole WPE takes 91.1-92.5 ms with it against
-  // 92.8-93.2 ms with the CUDA-core kernel: the DMMA build runs one CTA per SM (128 registers x 480
-  // threads), which leaves its serial prologue (load, lambda) unhidden and eats most of the fp64
-  // tensor cores' 2x rate.  The DFMA kernel stays the default; SETK_WPE_CORR=dmma selects the
-  // tensor-core build.
-  const int nblocks = wpe_dmma_blocks(a.NK, NA);
-  int dmma_warps = nblocks < 16 ? nblocks : 16;
-  int dmma_slots = (nblocks + dmma_warps - 1) / dmma_warps;
-  dmma_warps = (nblocks + dmma_slots - 1) / dmma_slots;
-  const int dmma_threads = 32 * dmma_warps;
-  {
-    const char* env = getenv("SETK_WPE_CORR");
-    if (!(env && strcmp(env, "dmma") == 0) || dmma_slots > 3) dmma_slots = 0;
-  }
   const int solve_threads = 4 * (((a.NK + 7) / 8) * 8);             // 4 column groups per row, whole warps
   const size_t solve_smem = sizeof(double) * (2 * (size_t)a.NK * (NA + 1) + 16) + sizeof(int) * 16;
 #ifndef SETK_EMU
   cudaError_t ea = cudaFuncSetAttribute(wpe_corr_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (ea == cudaSuccess)
-    ea = cudaFuncSetAttribute(wpe_corr_dmma_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (ea == cudaSuccess)
-    ea = cudaFuncSetAttribute(wpe_corr_dmma_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (ea == cudaSuccess)
-    ea = cudaFuncSetAttribute(wpe_corr_dmma_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (ea == cudaSuccess)
     ea = cudaFuncSetAttribute(wpe_filter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (ea == cudaSuccess)
@@ -513,14 +342,7 @@ cudaError_t run_wpe(const float2* X, int P, int B, int C, int F, int T, int taps
   cudaError_t e = cudaSuccess;
   for (int it = 0; it < num_iters && e == cudaSuccess; ++it) {
     a.use_filter = it > 0;
-    if (dmma_slots == 1)
-      e = launch(wpe_corr_dmma_kernel<1>, dim3(B * F), dim3(dmma_threads), smem, stream, false, a);
-    else if (dmma_slots == 2)
-      e = launch(wpe_corr_dmma_kernel<2>, dim3(B * F), dim3(dmma_threads), smem, stream, false, a);
-    else if (dmma_slots == 3)
-      e = launch(wpe_corr_dmma_kernel<3>, dim3(B * F), dim3(dmma_threads), smem, stream, false, a);
-    else
-      e = launch(wpe_corr_kernel, dim3(B * F), dim3(corr_threads), smem, stream, false, a);
+    e = launch(wpe_corr_kernel, dim3(B * F), dim3(corr_threads), smem, stream, false, a);
     if (e == cudaSuccess)
       e = launch(wpe_solve_kernel, dim3(B * F), dim3(solve_threads), solve_smem, stream, false, a, G);
   }

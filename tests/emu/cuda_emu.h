@@ -163,7 +163,6 @@ struct Ctx {
   std::mutex named_m;
   std::vector<uint64_t> slots;
   std::vector<float> gather;      // [nthreads][8]: warp all-gather scratch (emulated mma.sync)
-  std::vector<double> gather64;   // the same for fp64 fragments
   unsigned char* dyn = nullptr;
   bool serial = false;
 };
@@ -202,7 +201,6 @@ void launch(dim3 grid, dim3 block, size_t smem, bool serial, F&& body) {
         }
         ctx.slots.assign(nthr, 0);
         ctx.gather.assign((size_t)nthr * 8, 0.f);
-        ctx.gather64.assign((size_t)nthr * 4, 0.0);
         memset(dyn, 0xCD, smem);   // shared memory starts as garbage, like on the device
         auto run = [&](int tid) {
           g_ctx = &ctx; g_tid = tid;
@@ -251,17 +249,6 @@ inline void warp_allgather(const float* mine, int n, float* all) {
   for (int l = 0; l < 32; ++l) {
     const int src = w0 + l < g_ctx->nthreads ? w0 + l : g_tid;
     for (int i = 0; i < n; ++i) all[i * 32 + l] = buf[(size_t)src * 8 + i];
-  }
-  sync_warp();
-}
-inline void warp_allgather64(const double* mine, int n, double* all) {      // n <= 4
-  double* buf = g_ctx->gather64.data();
-  for (int i = 0; i < n; ++i) buf[(size_t)g_tid * 4 + i] = mine[i];
-  sync_warp();
-  const int w0 = g_tid & ~31;
-  for (int l = 0; l < 32; ++l) {
-    const int src = w0 + l < g_ctx->nthreads ? w0 + l : g_tid;
-    for (int i = 0; i < n; ++i) all[i * 32 + l] = buf[(size_t)src * 4 + i];
   }
   sync_warp();
 }

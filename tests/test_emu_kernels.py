@@ -69,20 +69,16 @@ def test_stft_cov_ws_protocol(emu, B, N, hop, center, with_mn, clip, mask_ft):
                       with_mask_n=with_mn, clip=clip, mask_ft=mask_ft)
 
 
-def test_stft_cov_ws_pair_window(emu, monkeypatch):
-    monkeypatch.setenv("SETK_WS_PAIRWIN", "1")       # opt-in: window folded into the first butterflies
-    pc.check_stft_cov(emu, np.random.default_rng(11), 2, 4, 3000)
-    pc.check_stft_cov(emu, np.random.default_rng(11), 2, 4, 3000, 512, 256, True, "hamming", with_mask_n=True)
-    pc.check_stft_cov(emu, np.random.default_rng(11), 1, 4, 3000, 400, 256, True, "hann")   # no pair sum: falls back
-
-
-def test_stft_cov_ws_direct_loads(emu, monkeypatch):
-    # opt-in: interior tiles' samples by global loads (no staging), edge tiles staged as before
-    monkeypatch.setenv("SETK_WS_AUDIO", "direct")
-    pc.check_stft_cov(emu, np.random.default_rng(12), 3, 4, 6000, clip=True)
-    pc.check_stft_cov(emu, np.random.default_rng(12), 2, 4, 5000, 512, 128, False, "hamming", with_mask_n=True)
-    ns = torch.tensor([3000, 200, 1701, 513, 2999, 256, 257, 1024], dtype=torch.int32)
-    pc.check_stft_cov(emu, np.random.default_rng(8), 8, 4, 3000, n_samples=ns)
+@pytest.mark.parametrize("B,N,fl,hop,center,window,with_mn,clip", [
+    (2, 3000, 512, 256, True, "hamming", True, False),   # a window other than Hann, mask_n rows
+    (2, 5000, 512, 128, False, "hamming", True, False),  # hop 128 without centring
+    (3, 6000, 512, 256, True, "hann", False, True),      # interior tiles between the padded edges, clip
+    (1, 3000, 400, 256, True, "hann", False, False),     # 400-sample frame zero-padded to 512
+])
+def test_stft_cov_ws_windows(emu, B, N, fl, hop, center, window, with_mn, clip):
+    # the warp-specialised build with other windows, frame lengths and lengths
+    pc.check_stft_cov(emu, np.random.default_rng(11), B, 4, N, fl, hop, center, window,
+                      with_mask_n=with_mn, clip=clip)
 
 
 def test_stft_cov_ws_long_run(emu):
@@ -184,6 +180,7 @@ def test_wpe(emu):
     pc.check_wpe(emu, rng, 2, 3, 2000, 256, 64, taps=4, delay=2, ctx=1, iters=2)
     pc.check_wpe(emu, rng, 1, 2, 2000, 256, 64, taps=6, delay=1, ctx=0, iters=1)
     pc.check_wpe(emu, rng, 1, 5, 3000, 256, 128, taps=3, delay=3, ctx=2, iters=2)   # NK = 15: ragged tiles
+    pc.check_wpe(emu, rng, 1, 3, 3000, 256, 64, taps=4, delay=2, ctx=1, iters=2)
 
 
 def test_wpe_chunked_long_utterance_path(emu, monkeypatch):
@@ -197,15 +194,6 @@ def test_wpe_chunked_long_utterance_path(emu, monkeypatch):
         out = pc.check_wpe(emu, rng, 1, 3, 2000, 256, 64, taps=4, delay=2, ctx=1, iters=2,
                            return_out=True)
         assert np.array_equal(out, ref)
-
-
-def test_wpe_tensor_core_correlation(emu, monkeypatch):
-    # SETK_WPE_CORR=dmma: the fp64 mma.sync build of the correlation pass (kept selectable; the
-    # CUDA-core kernel is the default)
-    monkeypatch.setenv("SETK_WPE_CORR", "dmma")
-    rng = np.random.default_rng(22)
-    pc.check_wpe(emu, rng, 1, 3, 3000, 256, 64, taps=4, delay=2, ctx=1, iters=2)
-    pc.check_wpe_fixture(emu, "c2_t6_ctx0")
 
 
 def test_wpe_reference_fixture(emu):
@@ -257,12 +245,8 @@ def test_weights_all_kinds(emu, C):
     pc.check_weights(emu, np.random.default_rng(10 + C), 2, 7, C)
 
 
-def test_weights_c4_thread_groups(emu, monkeypatch):
-    # C = 4 default: eigenvector kinds on 4 threads per problem, Cholesky kinds one thread per problem
-    monkeypatch.setenv("SETK_W_IMPL", "coop")         # every supported kind on thread groups
-    pc.check_weights(emu, np.random.default_rng(14), 2, 7, 4)
-    pc.check_weights_status(emu, C=4)
-    monkeypatch.setenv("SETK_W_IMPL", "thread")       # every kind on the one-thread kernels
+def test_weights_c4_thread_groups(emu):
+    # C = 4: eigenvector kinds on 4 threads per problem, Cholesky kinds one thread per problem
     pc.check_weights(emu, np.random.default_rng(14), 2, 7, 4)
     pc.check_weights_status(emu, C=4)
 

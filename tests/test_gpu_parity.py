@@ -61,6 +61,8 @@ def test_stft_cov_fused(cuda, C, N, hop, center, with_mn, clip, mask_ft):
 def test_stft_cov_fused_ragged(cuda):
     ns = torch.tensor([30000, 17001, 20480, 600], dtype=torch.int32)
     pc.check_stft_cov(cuda, np.random.default_rng(4), 4, 4, 30000, n_samples=ns)
+    ns = torch.tensor([30000, 19000, 9000], dtype=torch.int32)
+    pc.check_stft_cov(cuda, np.random.default_rng(41), 3, 4, 30000, n_samples=ns)
 
 
 def test_stft_cov_generic_route(cuda):
@@ -68,6 +70,7 @@ def test_stft_cov_generic_route(cuda):
     pc.check_stft_cov(cuda, np.random.default_rng(6), 2, 6, 9000, 512, 256, True, "hann",
                       with_mask_n=True)                                                        # config-4 channels
     pc.check_stft_cov(cuda, np.random.default_rng(7), 1, 16, 8000, 512, 256, True, "hann")
+    pc.check_stft_cov(cuda, np.random.default_rng(41), 2, 8, 20000)                          # tensor-core covariance
 
 
 @pytest.mark.parametrize("C", [5, 6, 8, 16])
@@ -100,6 +103,7 @@ def test_weights_all_kinds(cuda, C):
 
 def test_weights_c64_and_status(cuda):
     pc.check_weights(cuda, np.random.default_rng(20), 2, 64, 4, dtype=np.complex64)
+    pc.check_weights(cuda, np.random.default_rng(41), 3, 257, 4)     # every kind, a full set of bins
     pc.check_weights_status(cuda)
     pc.check_weights_status(cuda, C=6)         # the thread-group kernels of weights_coop.cu
     pc.check_weights_status(cuda, C=16)
@@ -123,32 +127,6 @@ def test_apply_istft_nsamps_and_ragged(cuda):
     pc.check_apply_istft(cuda, rng, 1, 4, 30000, n_out=20000)
     ns = torch.tensor([30000, 19000, 1000], dtype=torch.int32)
     pc.check_apply_istft(cuda, rng, 3, 4, 30000, n_samples=ns)
-
-
-def test_opt_in_builds(cuda, monkeypatch):
-    """Builds kept behind environment knobs stay correct: the classic fused STFT+covariance, the
-    pair-window / direct-load paths of the ws kernel, CUDA-core covariance, both weight-solve layouts
-    at C = 4."""
-    rng = np.random.default_rng(41)
-    ns = torch.tensor([30000, 19000, 9000], dtype=torch.int32)
-    for knob, val in (("SETK_SC_IMPL", "classic"), ("SETK_WS_PAIRWIN", "1"), ("SETK_WS_AUDIO", "direct")):
-        monkeypatch.setenv(knob, val)
-        pc.check_stft_cov(cuda, rng, 3, 4, 30000, n_samples=ns)
-        monkeypatch.delenv(knob)
-    monkeypatch.setenv("SETK_COV_IMPL", "cuda")
-    pc.check_stft_cov(cuda, rng, 2, 8, 20000)
-    monkeypatch.delenv("SETK_COV_IMPL")
-    for impl in ("coop", "thread"):
-        monkeypatch.setenv("SETK_W_IMPL", impl)
-        pc.check_weights(cuda, rng, 3, 257, 4)
-        monkeypatch.delenv("SETK_W_IMPL")
-
-
-def test_wpe_tensor_core_correlation(cuda, monkeypatch):
-    """SETK_WPE_CORR=dmma: the mma.sync.m8n8k4.f64 build of wpe_step's R, r (libs/wpe.py:58-77)."""
-    monkeypatch.setenv("SETK_WPE_CORR", "dmma")
-    pc.check_wpe(cuda, np.random.default_rng(22), 2, 6, 16000, 512, 128, taps=10, delay=3, ctx=1, iters=2)
-    pc.check_wpe_fixture(cuda, "c2_t6_ctx0")
 
 
 def test_non_power_of_two_n_fft(cuda):
@@ -343,6 +321,7 @@ def test_cgmm_documented_command_from_audio(cuda, which):
 @pytest.mark.parametrize("C,fl,hop,taps,delay,ctx,iters,N", [
     (6, 512, 256, 10, 3, 1, 3, 48000),      # config-4 geometry: NK = 60
     (8, 512, 128, 10, 3, 1, 2, 24000),      # NK = 80
+    (6, 512, 128, 10, 3, 1, 2, 16000),
     (2, 1024, 256, 12, 2, 0, 1, 30000),
     (5, 512, 128, 3, 3, 2, 3, 16000),       # NK = 15: ragged tiles
     (1, 512, 128, 10, 3, 1, 3, 16000),
