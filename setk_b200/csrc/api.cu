@@ -1,6 +1,7 @@
 // api.cu -- the C-ABI of libsetk_b200.so (include/setk_b200.h): argument
 // checking, plan / workspace management and dispatch to the kernels.
 #include "common.cuh"
+#include "launchers.cuh"
 
 #include <math.h>
 #include <stdarg.h>
@@ -13,75 +14,6 @@
 namespace setk {
 
 std::atomic<long long> g_launch_count{0};
-
-// --- launchers implemented in the other translation units ---
-cudaError_t run_stft_generic(const setk_plan*, const float*, const int*, int, int, int, float2*, void*);
-cudaError_t run_cov_generic(const float2*, const float*, unsigned, int, int, int, int, float2*, void*);
-cudaError_t run_apply_generic(const float2*, const void*, int, const float*, int, int, int, int, float2*, void*);
-cudaError_t run_istft_generic(const setk_plan*, const float2*, int, int, int, int, const int*, float*, float*,
-                              unsigned*, void*);
-cudaError_t run_peak_scale(float*, int, int, const float*, const unsigned*, void*);
-cudaError_t run_float_to_pcm16(const float*, long long, int16_t*, void*);
-cudaError_t run_peak_scale_pcm16(const float*, int, int, const float*, const unsigned*, int16_t*, void*);
-cudaError_t run_pcm16_to_float(const int16_t*, long long, float*, void*);
-cudaError_t run_cm_masks(const unsigned char*, long long, int, int, int, float*, int*, void*);
-
-cudaError_t run_ipd(const float2*, const float2*, long long, int, int, float*, void*);
-cudaError_t run_dirfeat(const float2*, const double2*, int, const int*, int, int, int, int, int, double*,
-                        void*);
-size_t gcc_phat_work_doubles(int, int, int);
-cudaError_t run_gcc_phat(const float2*, const float2*, int, int, const double*, const double*, int, int,
-                         int, int, double*, double*, void*);
-size_t msc_work_doubles(int, int);
-cudaError_t run_msc(const float2*, int, int, int, int, int, double*, double*, void*);
-bool stft_cov_fused_supported(const Geometry&);
-size_t stft_cov_partial_floats(const Geometry&);
-size_t stft_cov_partial_bytes(const setk_plan*, int, int);
-int stft_cov_pick_chunks(const setk_plan*, int, int);
-cudaError_t run_stft_cov_fused(setk_plan*, const float*, const int*, int, int, int, const float*,
-                               const float*, unsigned, int*, float*, unsigned*, float2*, float2*, float*,
-                               void*);
-bool apply_istft_fused_supported(const Geometry&);
-cudaError_t run_apply_istft_fused(setk_plan*, const float*, const int*, int, int, int, const void*, int,
-                                  const float*, int, int*, float*, unsigned*, void*);
-
-bool stft_spill_supported(const Geometry&);
-size_t stft_spill_bytes(const Geometry&, int, int);
-size_t apply_spill_bytes(const Geometry&, int, int);
-cudaError_t run_spill_to_bcft(const setk_plan*, const float2*, int, int, float2*, void*);
-struct CgCtx { Geometry geo; int sm_count; };
-size_t cgmm_workspace_bytes(const CgCtx*, int, int, int, int);
-cudaError_t run_cgmm(const CgCtx*, const float2*, int, double*, const int*, int, int, int, int, int, const float*,
-                     int, float*, unsigned*, void*);
-cudaError_t run_bcft_to_spill(const float2*, int, int, int, int, int, float2*, void*);
-bool wpe_supported(int, int, int, int, int);
-size_t wpe_workspace_bytes(int, int, int, int);
-cudaError_t run_wpe(const float2*, int, int, int, int, int, int, int, int, int, double*, float2*, unsigned*,
-                    const float2*, float*, void*);
-cudaError_t run_apply_spill(setk_plan*, const float2*, const void*, int, const float*, int, int, float2*, void*);
-cudaError_t run_istft_strided(const setk_plan*, const float2*, long long, long long, long long, int, int, int,
-                              const int*, float*, float*, unsigned*, void*);
-size_t cov_spill_partial_bytes(const Geometry&, int, int);
-int cov_spill_chunks(const setk_plan*, int, int);
-cudaError_t run_stft_spill(setk_plan*, const float*, const int*, int, int, int, int, float2*, unsigned*,
-                           void*);
-cudaError_t run_cov_spill(setk_plan*, const float2*, const float*, const float*, unsigned, const int*,
-                          int, int, int, int, float*, float2*, float2*, void*);
-cudaError_t run_bits_to_float(const unsigned*, int, float*, void*);
-size_t ssl_scratch_bytes(int, int, int, int, int, int, int, int, int);
-cudaError_t run_ssl(int, const float2*, int, int, int, int, const double2*, int, const float*, int, const int*,
-                    int, const int*, int, double, double, int, char*, double*, int*, void*);
-size_t auxiva_scratch_bytes(int, int, int, int);
-cudaError_t run_auxiva(const float2*, int, int, int, int, int, char*, double2*, unsigned*, void*);
-
-struct WeightsArgs;
-cudaError_t weights_run(int kind, double beta, int ref_channel, int rank1, int ban, const void* Rs,
-                        const void* Rn, const void* Ry, int r_dtype, int B, int F, int C, void* w,
-                        int w_dtype, unsigned* status, int* ref_used, void* stream);
-cudaError_t maxabs_generic(const float* audio, const int* n_samples, int B, int C, int N,
-                           unsigned* bits, float* out, void* stream);
-cudaError_t post_run(int mode, const void* A, const void* Rn, int dtype, int B, int F, int C, void* out,
-                     unsigned* status, void* stream);
 
 static thread_local char g_err[512] = "";
 
@@ -109,6 +41,35 @@ static cudaError_t ensure(T** ptr, size_t* have, size_t want) {
 }
 
 static bool is_pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
+
+// Tile STFT of the batch into the plan's bin-major workspace d_stft_ws [B][T][C][bin_pitch(F)]
+// (stft_spill.cu), with max|x| per utterance into maxabs_bits unless that is null.  A failure is
+// reported as ws_what when the workspace cannot grow, as run_what when the launch fails.
+static int stft_to_bin_major(setk_plan* pl, const float* audio, const int32_t* n_samples, int B, int N, int T,
+                             unsigned* maxabs_bits, void* stream, const char* ws_what, const char* run_what) {
+  const Geometry& g = pl->geo;
+  cudaError_t e = ensure(&pl->d_stft_ws, &pl->stft_ws_bytes, stft_spill_bytes(g, B, T));
+  if (e != cudaSuccess) return cuda_fail(e, ws_what);
+  const int groups = (g.C + 3) / 4;   // the kernels take channels in groups of <= 4
+  e = run_stft_spill(pl, audio, n_samples, B, N, T, stft_cov_pick_chunks(pl, B * groups, T), pl->d_stft_ws,
+                     maxabs_bits, stream);
+  return e == cudaSuccess ? SETK_OK : cuda_fail(e, run_what);
+}
+
+// Runs run(scratch) with `bytes` of scratch allocated on the caller's stream (cudaMallocAsync /
+// cudaFreeAsync), so that the plan-free entry points share no memory between calls on different
+// streams or devices.  A failed free is reported only when the run itself succeeded.
+template <class Run>
+static int with_scratch(size_t bytes, void* stream, const char* alloc_what, const char* run_what, Run run) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  char* ws = nullptr;
+  cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&ws), bytes, st);
+  if (e != cudaSuccess) return cuda_fail(e, alloc_what);
+  e = run(ws);
+  const cudaError_t ef = cudaFreeAsync(ws, st);
+  if (e == cudaSuccess) e = ef;
+  return e == cudaSuccess ? SETK_OK : cuda_fail(e, run_what);
+}
 
 }  // namespace setk
 
@@ -229,13 +190,9 @@ int setk_stft(setk_plan_t* pl, const float* audio, const int32_t* n_samples, int
   cudaError_t e;
   if (stft_spill_supported(g) && (long long)B * g.C <= 65535) {
     // tile STFT into the bin-major workspace, then one transposing copy
-    e = ensure(&pl->d_stft_ws, &pl->stft_ws_bytes, stft_spill_bytes(g, B, T));
-    if (e != cudaSuccess) return cuda_fail(e, "setk_stft(workspace)");
-    const int groups = (g.C + 3) / 4;
-    e = run_stft_spill(pl, audio, n_samples, B, N, T, stft_cov_pick_chunks(pl, B * groups, T), pl->d_stft_ws,
-                       nullptr, stream);
-    if (e == cudaSuccess)
-      e = run_spill_to_bcft(pl, pl->d_stft_ws, B, T, static_cast<float2*>(stft_out), stream);
+    rc = stft_to_bin_major(pl, audio, n_samples, B, N, T, nullptr, stream, "setk_stft(workspace)", "setk_stft");
+    if (rc) return rc;
+    e = run_spill_to_bcft(pl, pl->d_stft_ws, B, T, static_cast<float2*>(stft_out), stream);
   } else {
     e = run_stft_generic(pl, audio, n_samples, B, N, T, static_cast<float2*>(stft_out), stream);
   }
@@ -282,18 +239,15 @@ int setk_stft_cov(setk_plan_t* pl, const float* audio, const int32_t* n_samples,
   if (stft_spill_supported(g)) {
     // many-channel route (C > 4 at n_fft = 512, any C at n_fft = 1024): fast STFT
     // into a bin-major workspace, then a streaming covariance kernel (stft_spill.cu)
-    const int groups = (g.C + 3) / 4;
-    const int chunks_a = stft_cov_pick_chunks(pl, B * groups, T);
     // >= 16 short fp32 runs per utterance, combined in double by the finalize kernel
-    const int chunks_b = cov_spill_chunks(pl, B, T);
-    e = ensure(&pl->d_stft_ws, &pl->stft_ws_bytes, stft_spill_bytes(g, B, T));
-    if (e == cudaSuccess)
-      e = ensure(&pl->d_partials, &pl->partials_bytes, cov_spill_partial_bytes(g, B, chunks_b));
+    const int chunks = cov_spill_chunks(pl, B, T);
+    e = ensure(&pl->d_partials, &pl->partials_bytes, cov_spill_partial_bytes(g, B, chunks));
     if (e != cudaSuccess) return cuda_fail(e, "setk_stft_cov(workspace)");
-    e = run_stft_spill(pl, audio, n_samples, B, N, T, chunks_a, pl->d_stft_ws, maxabs_bits, stream);
-    if (e == cudaSuccess)
-      e = run_cov_spill(pl, pl->d_stft_ws, mask_s, mask_n, flags, n_samples, B, N, T, chunks_b,
-                        pl->d_partials, static_cast<float2*>(Rs), static_cast<float2*>(Rn), stream);
+    rc = stft_to_bin_major(pl, audio, n_samples, B, N, T, maxabs_bits, stream, "setk_stft_cov(workspace)",
+                           "setk_stft_cov(spill)");
+    if (rc) return rc;
+    e = run_cov_spill(pl, pl->d_stft_ws, mask_s, mask_n, flags, n_samples, B, N, T, chunks, pl->d_partials,
+                      static_cast<float2*>(Rs), static_cast<float2*>(Rn), stream);
     if (e == cudaSuccess && maxabs) e = run_bits_to_float(maxabs_bits, B, maxabs, stream);
     return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_stft_cov(spill)");
   }
@@ -366,18 +320,13 @@ int setk_apply(const void* stft, const void* w, int32_t w_dtype, const float* po
   return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_apply");
 }
 
-static int T_used_for(const Geometry& g, int T, int n_out) {
-  const int cap = (n_out + 2 * g.pad + g.hop - 1) / g.hop;
-  return T < cap ? T : cap;
-}
-
 int setk_istft(setk_plan_t* pl, const void* enh, int32_t B, int32_t T, int32_t n_out, const float* norm,
                float* wave, void* stream) {
   if (!pl || !enh || !wave) return fail(SETK_EINVAL, "setk_istft: null argument");
   if (B < 1 || B > pl->cfg.max_batch || T < 1 || n_out < 1)
     return fail(SETK_ESHAPE, "setk_istft: bad shape B=%d T=%d n_out=%d", B, T, n_out);
   const Geometry& g = pl->geo;
-  const int T_used = T_used_for(g, T, n_out);
+  const int T_used = imin(T, istft_frame_cap(g, n_out));
   cudaError_t e = ensure(&pl->d_frames_ws, &pl->frames_ws_bytes, sizeof(float) * (size_t)B * T_used * g.n_fft);
   if (e == cudaSuccess) e = ensure(&pl->d_peak, &pl->peak_bytes, sizeof(unsigned) * 2 * (size_t)pl->cfg.max_batch);
   if (e != cudaSuccess) return cuda_fail(e, "setk_istft(workspace)");
@@ -403,6 +352,7 @@ static int apply_istft_impl(setk_plan_t* pl, const float* audio, const int32_t* 
   if (n_out < 1) return fail(SETK_ESHAPE, "setk_apply_istft: n_out=%d", n_out);
   const Geometry& g = pl->geo;
   const int T = frames_of(N, g.n_fft, g.hop, g.pad);
+  const int T_used = imin(T, istft_frame_cap(g, n_out));   // the workspace routes' iSTFT
   cudaError_t e = ensure(&pl->d_peak, &pl->peak_bytes, sizeof(unsigned) * 2 * (size_t)pl->cfg.max_batch);
   if (e == cudaSuccess && pcm) {
     e = ensure(&pl->d_wave_ws, &pl->wave_ws_bytes, sizeof(float) * (size_t)B * n_out);
@@ -423,23 +373,18 @@ static int apply_istft_impl(setk_plan_t* pl, const float* audio, const int32_t* 
   } else if (stft_spill_supported(g)) {
     // tile STFT into the bin-major workspace, y = w^H x over it, then the
     // frame-wise inverse FFT + overlap-add reading Y[b][t][f] in place
-    const int T_used = T_used_for(g, T, n_out);
-    const int groups = (g.C + 3) / 4;
-    const int chunks = stft_cov_pick_chunks(pl, B * groups, T);
-    const long long pitch = (long long)(apply_spill_bytes(g, 1, 1) / sizeof(float2));
-    e = ensure(&pl->d_stft_ws, &pl->stft_ws_bytes, stft_spill_bytes(g, B, T));
-    if (e == cudaSuccess) e = ensure(&pl->d_enh_ws, &pl->enh_ws_bytes, apply_spill_bytes(g, B, T));
+    const long long pitch = bin_pitch(g.F);
+    e = ensure(&pl->d_enh_ws, &pl->enh_ws_bytes, apply_spill_bytes(g, B, T));
     if (e == cudaSuccess)
       e = ensure(&pl->d_frames_ws, &pl->frames_ws_bytes, sizeof(float) * (size_t)B * T_used * g.n_fft);
-    if (e == cudaSuccess)
-      e = run_stft_spill(pl, audio, n_samples, B, N, T, chunks, pl->d_stft_ws, nullptr, stream);
-    if (e == cudaSuccess)
-      e = run_apply_spill(pl, pl->d_stft_ws, w, w_dtype, post_mask, B, T, pl->d_enh_ws, stream);
+    if (e != cudaSuccess) return cuda_fail(e, "setk_apply_istft");
+    rc = stft_to_bin_major(pl, audio, n_samples, B, N, T, nullptr, stream, "setk_apply_istft", "setk_apply_istft");
+    if (rc) return rc;
+    e = run_apply_spill(pl, pl->d_stft_ws, w, w_dtype, post_mask, B, T, pl->d_enh_ws, stream);
     if (e == cudaSuccess)
       e = run_istft_strided(pl, pl->d_enh_ws, (long long)T * pitch, 1, pitch, B, T_used, n_out, n_samples,
                             pl->d_frames_ws, wave, peak, stream);
   } else {
-    const int T_used = T_used_for(g, T, n_out);
     e = ensure(&pl->d_stft_ws, &pl->stft_ws_bytes, sizeof(float2) * (size_t)B * g.C * g.F * T);
     if (e == cudaSuccess) e = ensure(&pl->d_enh_ws, &pl->enh_ws_bytes, sizeof(float2) * (size_t)B * g.F * T);
     if (e == cudaSuccess)
@@ -489,19 +434,16 @@ int setk_cgmm_masks(setk_plan_t* pl, const float* audio, const int32_t* n_sample
     return fail(SETK_EUNSUPPORTED, "setk_cgmm_masks: needs n_fft 512 or 1024 (got %d, hop %d)", g.n_fft, g.hop);
   const int T = frames_of(N, g.n_fft, g.hop, g.pad);
   if (T < 1) return fail(SETK_ESHAPE, "setk_cgmm_masks: no frame in %d samples", N);
-  const int P = (int)(apply_spill_bytes(g, 1, 1) / sizeof(float2));
+  const int P = bin_pitch(g.F);
   CgCtx ctx;
   ctx.geo = g; ctx.sm_count = pl->sm_count;
-  cudaError_t e = ensure(&pl->d_stft_ws, &pl->stft_ws_bytes, stft_spill_bytes(g, B, T));
-  if (e == cudaSuccess)
-    e = ensure(&pl->d_cgmm_ws, &pl->cgmm_ws_bytes, cgmm_workspace_bytes(&ctx, B, T, num_classes, P));
+  cudaError_t e = ensure(&pl->d_cgmm_ws, &pl->cgmm_ws_bytes, cgmm_workspace_bytes(&ctx, B, T, num_classes, P));
   if (e != cudaSuccess) return cuda_fail(e, "setk_cgmm_masks(workspace)");
-  const int groups = (g.C + 3) / 4;
-  e = run_stft_spill(pl, audio, n_samples, B, N, T, stft_cov_pick_chunks(pl, B * groups, T), pl->d_stft_ws,
-                     nullptr, stream);
-  if (e == cudaSuccess)
-    e = run_cgmm(&ctx, pl->d_stft_ws, P, pl->d_cgmm_ws, n_samples, B, N, T, num_classes, num_iters, init_gamma,
-                 update_alpha, masks, status, stream);
+  rc = stft_to_bin_major(pl, audio, n_samples, B, N, T, nullptr, stream, "setk_cgmm_masks(workspace)",
+                         "setk_cgmm_masks");
+  if (rc) return rc;
+  e = run_cgmm(&ctx, pl->d_stft_ws, P, pl->d_cgmm_ws, n_samples, B, N, T, num_classes, num_iters, init_gamma,
+               update_alpha, masks, status, stream);
   return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_cgmm_masks");
 }
 
@@ -524,22 +466,19 @@ int setk_cgmm_stft(const void* stft, int32_t B, int32_t C, int32_t F, int32_t T,
   cudaError_t e = cudaGetDevice(&dev);
   if (e == cudaSuccess) e = cudaDeviceGetAttribute(&ctx.sm_count, cudaDevAttrMultiProcessorCount, dev);
   if (e != cudaSuccess) return cuda_fail(e, "setk_cgmm_stft(device)");
-  const int P = (F + 7) & ~7;
+  // scratch: the bin-major copy X of the STFT, then (256-byte aligned) the CGMM workspace
+  const int P = bin_pitch(F);
   const size_t x_bytes = sizeof(float2) * (size_t)B * T * C * P;
   const size_t w_bytes = cgmm_workspace_bytes(&ctx, B, T, num_classes, P);
-  char* ws = nullptr;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  e = cudaMallocAsync(reinterpret_cast<void**>(&ws), x_bytes + w_bytes + 256, st);   // stream-ordered scratch
-  if (e != cudaSuccess) return cuda_fail(e, "setk_cgmm_stft(workspace)");
-  float2* X = reinterpret_cast<float2*>(ws);
-  double* cw = reinterpret_cast<double*>(ws + ((x_bytes + 255) / 256) * 256);
-  e = run_bcft_to_spill(static_cast<const float2*>(stft), B, C, F, T, P, X, stream);
-  if (e == cudaSuccess)
-    e = run_cgmm(&ctx, X, P, cw, nullptr, B, /*N=*/T + 1, T, num_classes, num_iters, init_gamma, update_alpha,
-                 masks, status, stream);
-  cudaError_t ef = cudaFreeAsync(ws, st);
-  if (e == cudaSuccess) e = ef;
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_cgmm_stft");
+  return with_scratch(x_bytes + w_bytes + 256, stream, "setk_cgmm_stft(workspace)", "setk_cgmm_stft",
+                      [&](char* ws) {
+    float2* X = reinterpret_cast<float2*>(ws);
+    cudaError_t e = run_bcft_to_spill(static_cast<const float2*>(stft), B, C, F, T, P, X, stream);
+    if (e == cudaSuccess)
+      e = run_cgmm(&ctx, X, P, reinterpret_cast<double*>(ws + up256(x_bytes)), nullptr, B, /*N=*/T + 1, T,
+                   num_classes, num_iters, init_gamma, update_alpha, masks, status, stream);
+    return e;
+  });
 }
 
 static int wpe_entry(const char* who, const void* stft, const void* lambda_enh, int32_t B, int32_t C, int32_t F,
@@ -554,22 +493,18 @@ static int wpe_entry(const char* who, const void* stft, const void* lambda_enh, 
   if (!wpe_supported(C, T, taps, delay, context))
     return fail(SETK_EUNSUPPORTED, "%s: %d channels x %d taps (context %d) exceeds the kernels' "
                 "shared-memory budget", who, C, taps, context);
-  const int P = (F + 7) & ~7;
+  // scratch: the bin-major copy X of the STFT, then (256-byte aligned) the WPE workspace
+  const int P = bin_pitch(F);
   const size_t x_bytes = sizeof(float2) * (size_t)B * T * C * P;
   const size_t w_bytes = wpe_workspace_bytes(B, C, F, taps);
-  char* ws = nullptr;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&ws), x_bytes + w_bytes + 256, st);
-  if (e != cudaSuccess) return cuda_fail(e, who);
-  float2* X = reinterpret_cast<float2*>(ws);
-  double* dw = reinterpret_cast<double*>(ws + ((x_bytes + 255) / 256) * 256);
-  e = run_bcft_to_spill(static_cast<const float2*>(stft), B, C, F, T, P, X, stream);
-  if (e == cudaSuccess)
-    e = run_wpe(X, P, B, C, F, T, taps, delay, context, num_iters, dw, static_cast<float2*>(out), status,
-                static_cast<const float2*>(lambda_enh), inv_lambda, stream);
-  cudaError_t ef = cudaFreeAsync(ws, st);
-  if (e == cudaSuccess) e = ef;
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, who);
+  return with_scratch(x_bytes + w_bytes + 256, stream, who, who, [&](char* ws) {
+    float2* X = reinterpret_cast<float2*>(ws);
+    cudaError_t e = run_bcft_to_spill(static_cast<const float2*>(stft), B, C, F, T, P, X, stream);
+    if (e == cudaSuccess)
+      e = run_wpe(X, P, B, C, F, T, taps, delay, context, num_iters, reinterpret_cast<double*>(ws + up256(x_bytes)),
+                  static_cast<float2*>(out), status, static_cast<const float2*>(lambda_enh), inv_lambda, stream);
+    return e;
+  });
 }
 
 int setk_wpe_stft(const void* stft, int32_t B, int32_t C, int32_t F, int32_t T, int32_t taps, int32_t delay,
@@ -692,16 +627,11 @@ int setk_ssl(int32_t backend, const void* stft, int32_t B, int32_t M, int32_t F,
       return fail(SETK_EINVAL, "setk_ssl: window [%d, %d) of utterance %lld outside [0, %d] or empty", s, e,
                   i / W, T);
   }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  char* ws = nullptr;
-  cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&ws), ssl_scratch_bytes(backend, B, N, M, F, T, A, W, P),
-                                  st);   // stream-ordered scratch
-  if (e != cudaSuccess) return cuda_fail(e, "setk_ssl(workspace)");
-  e = run_ssl(backend, static_cast<const float2*>(stft), B, M, F, T, static_cast<const double2*>(steer), A, mask,
-              N, windows_host, W, pairs_host, P, compression, eps, normalize, ws, scores, index, stream);
-  cudaError_t ef = cudaFreeAsync(ws, st);
-  if (e == cudaSuccess) e = ef;
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_ssl");
+  return with_scratch(ssl_scratch_bytes(backend, B, N, M, F, T, A, W, P), stream, "setk_ssl(workspace)", "setk_ssl",
+                      [&](char* ws) {
+    return run_ssl(backend, static_cast<const float2*>(stft), B, M, F, T, static_cast<const double2*>(steer), A,
+                   mask, N, windows_host, W, pairs_host, P, compression, eps, normalize, ws, scores, index, stream);
+  });
 }
 
 // ---- AuxIVA blind source separation (auxiva.cuh, built in wpe.cu) ----
@@ -713,15 +643,11 @@ int setk_auxiva_stft(const void* stft, int32_t B, int32_t N, int32_t F, int32_t 
   if (num_epochs < 0) return fail(SETK_EINVAL, "setk_auxiva_stft: num_epochs=%d", num_epochs);
   if (B < 1 || F < 1 || T < 1 || B > 65535 || (long long)B * F > 2000000000LL)
     return fail(SETK_EINVAL, "setk_auxiva_stft: bad shape B=%d F=%d T=%d", B, F, T);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  char* ws = nullptr;
-  cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&ws), auxiva_scratch_bytes(B, N, F, T), st);
-  if (e != cudaSuccess) return cuda_fail(e, "setk_auxiva_stft(workspace)");
-  e = run_auxiva(static_cast<const float2*>(stft), B, N, F, T, num_epochs, ws, static_cast<double2*>(out),
-                 status, stream);
-  cudaError_t ef = cudaFreeAsync(ws, st);
-  if (e == cudaSuccess) e = ef;
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_auxiva_stft");
+  return with_scratch(auxiva_scratch_bytes(B, N, F, T), stream, "setk_auxiva_stft(workspace)", "setk_auxiva_stft",
+                      [&](char* ws) {
+    return run_auxiva(static_cast<const float2*>(stft), B, N, F, T, num_epochs, ws, static_cast<double2*>(out),
+                      status, stream);
+  });
 }
 
 }  // extern "C"

@@ -38,6 +38,7 @@
 #include "common.cuh"
 #include "stft_tile.cuh"
 #include "apply_istft_args.cuh"
+#include "launchers.cuh"
 
 namespace setk {
 
@@ -421,37 +422,23 @@ bool apply_istft_fused_supported(const Geometry& g) {
   return true;
 }
 
-void fused_schedule(const setk_plan* pl, int B, int T, int TT, int* n_ctas, int* slots, int* min_quota);
 // Warp-specialised builds of this pass (FFT / apply+flush / inverse-FFT roles on mbarrier rings) were
 // slower than this kernel (DESIGN.md K4+K5): four short stages per frame make the hand-overs cost more
 // than the two barriers they replace.  They are not part of the library.
-cudaError_t run_tile_prefix(const int* n_samples, int B, const Geometry& g, int TT, int T_cap,
-                            int* prefix, void* stream);
-
 cudaError_t run_apply_istft_fused(setk_plan* pl, const float* audio, const int* n_samples, int B, int N,
                                   int T, const void* w, int w_dtype, const float* post_mask, int n_out,
                                   int* tile_prefix, float* wave, unsigned* peak, void* stream) {
   constexpr int TT = 4;
-  const int TTs = TT;                                 // frames per tile of the schedule
   ApplyIstftArgs a;
   a.g = pl->geo;
   a.audio = audio; a.n_samples = n_samples; a.N = N;
   a.w = w; a.w_dtype = w_dtype;
   a.post_mask = post_mask; a.T = T;
   // persistent schedule over the frames librosa.istft uses for this output length
-  const int T_cap = (n_out + 2 * a.g.pad + a.g.hop - 1) / a.g.hop;
-  const int T_used = T < T_cap ? T : T_cap;
   int n_ctas, slots_unused;
-  fused_schedule(pl, B, T_used, TTs, &n_ctas, &slots_unused, &a.sched.min_quota);
-  a.sched.B = B;
-  a.sched.tiles_u = sched_tiles_of(T_used, TTs);
-  a.sched.prefix = nullptr;
-  cudaError_t e = cudaSuccess;
-  if (n_samples) {     // ragged batch: the lengths live on the device
-    e = run_tile_prefix(n_samples, B, pl->geo, TTs, T_cap, tile_prefix, stream);
-    if (e != cudaSuccess) return e;
-    a.sched.prefix = tile_prefix;
-  }
+  cudaError_t e = fused_schedule(pl, B, T, TT, istft_frame_cap(a.g, n_out), n_samples, tile_prefix, stream,
+                                 &a.sched, &n_ctas, &slots_unused);
+  if (e != cudaSuccess) return e;
   a.window = pl->d_window;
   a.wsq = pl->d_wsq;
   a.n_out = n_out;

@@ -25,6 +25,7 @@
 // Built in wpe.cu's translation unit (the other fp64 per-bin iterative front end).
 #pragma once
 #include "common.cuh"
+#include "launchers.cuh"
 #include "lu_coop.cuh"
 
 namespace setk {

@@ -25,6 +25,7 @@
 #include "async_copy.cuh"
 #include "common.cuh"
 #include "jacobi_coop.cuh"
+#include "launchers.cuh"
 
 namespace setk {
 
@@ -502,8 +503,6 @@ __global__ void __launch_bounds__(256) bcft_to_spill_kernel(const float2* __rest
 // ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
-struct CgCtx { Geometry geo; int sm_count; };
-
 cudaError_t run_bcft_to_spill(const float2* in, int B, int C, int F, int T, int P, float2* xws, void* stream) {
   return launch(bcft_to_spill_kernel, dim3((T + 31) / 32, (F + 31) / 32, B * C), dim3(256), 0, stream, false,
                 in, P, C, F, T, xws);

@@ -16,6 +16,7 @@
 // operation a float32 operation in the reference's order (numpy float32 arrays x weak python
 // scalars): no FMA contraction, IEEE division -- the result is bit-identical to the reference's.
 #include "common.cuh"
+#include "launchers.cuh"
 
 namespace setk {
 

@@ -33,6 +33,17 @@ SETK_HD inline int frames_of(int n, int n_fft, int hop, int pad) {
   return 1 + (padded - n_fft) / hop;
 }
 
+// frames of the STFT that librosa.istft reads for an n_out-sample output; a T-frame input uses
+// min(T, this) of its frames (the ones after them reach only trimmed samples)
+inline int istft_frame_cap(const Geometry& g, int n_out) { return (n_out + 2 * g.pad + g.hop - 1) / g.hop; }
+
+// row pitch (complex values) of the bin-major STFT workspaces [B][T][C][pitch]: F rounded up to a
+// multiple of 8 -- 264 for 257 bins (n_fft 512), 520 for 513 (n_fft 1024)
+SETK_HD constexpr int bin_pitch(int F) { return (F + 7) & ~7; }
+
+// n rounded up to a multiple of 256: the alignment of the regions carved from one scratch allocation
+inline size_t up256(size_t n) { return (n + 255) / 256 * 256; }
+
 // index into the un-padded signal of padded position p (np.pad mode="reflect")
 SETK_HD inline int reflect_index(int p, int pad, int n) {
   int i = p - pad;

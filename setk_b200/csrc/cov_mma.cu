@@ -31,6 +31,7 @@
 #include "common.cuh"
 #include "async_copy.cuh"
 #include "cov_spill_args.cuh"
+#include "launchers.cuh"
 #include "mma_tf32.cuh"
 
 namespace setk {

@@ -6,6 +6,7 @@
 // implementation with the reference's array layouts; the batch hot path uses
 // the fused kernels in stft_cov_fused.cu / apply_istft_fused.cu instead.
 #include "common.cuh"
+#include "launchers.cuh"
 
 namespace setk {
 

@@ -15,6 +15,7 @@
 // in float32 like the reference (np.angle of complex64), everything the
 // reference promotes to float64 (the GCC transform, MSC) is float64 here too.
 #include "common.cuh"
+#include "launchers.cuh"
 #include <math.h>
 
 namespace setk {

@@ -32,6 +32,7 @@
 // spatial analysis that turns these features into a direction.
 #pragma once
 #include "common.cuh"
+#include "launchers.cuh"
 #include <math.h>
 
 namespace setk {
@@ -295,12 +296,7 @@ __global__ void ssl_music_score_kernel(const double2* __restrict__ sv, const dou
   scores[i] = acc;
 }
 
-cudaError_t weights_run(int kind, double beta, int ref_channel, int rank1, int ban, const void* Rs,
-                        const void* Rn, const void* Ry, int r_dtype, int B, int F, int C, void* w,
-                        int w_dtype, unsigned* status, int* ref_used, void* stream);
-
 static unsigned blocks_of(long long n, int bs) { return (unsigned)((n + bs - 1) / bs); }
-static size_t up256(size_t n) { return (n + 255) / 256 * 256; }
 
 // Scratch (stream-ordered): device copies of the windows / pairs, then the backend's tables.
 size_t ssl_scratch_bytes(int backend, int B, int N, int M, int F, int T, int A, int W, int P) {

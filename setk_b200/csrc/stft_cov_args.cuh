@@ -6,6 +6,12 @@
 
 namespace setk {
 
+// frames per tile of the fused pass at C channels.  5 at C = 2: 320 threads, 10 FFT warps (the tenth
+// warp's registers are allocated either way at 288).  4 at odd C, where 5 would leave an odd number
+// of half-warp jobs, and at C = 4, whose warp-specialised build runs 16 half-warp jobs per tile.
+// The partial-sum workspace is sized and the kernels are launched with this schedule.
+constexpr int stft_cov_tt(int C) { return C == 2 ? 5 : 4; }
+
 template <int C>
 struct CovAcc {
   static constexpr int NOFF = C * (C - 1) / 2;

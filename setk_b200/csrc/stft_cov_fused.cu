@@ -29,6 +29,7 @@
 #include "common.cuh"
 #include "stft_tile.cuh"
 #include "stft_cov_args.cuh"
+#include "launchers.cuh"
 
 namespace setk {
 
@@ -36,9 +37,6 @@ namespace setk {
 // register file (allocation granularity: 2 warps), so two CTAs per SM need
 // <= 65536 / (2 * 10 * 32) = 102 -> 96 registers (ncu: 112 left ONE CTA per SM)
 constexpr int kScRegs = 96;
-// frames per tile at even C: 4 -> 288 threads (8 FFT warps + the Nyquist warp), 5 -> 320 threads
-// (10 FFT warps: the tenth warp's registers are allocated either way)
-constexpr int kScTT = 5;
 
 // tiles before every utterance of a ragged batch (one CTA; B is small)
 __global__ void tile_prefix_kernel(const int* __restrict__ n_samples, int B, Geometry g, int TT,
@@ -67,12 +65,6 @@ __global__ void tile_prefix_kernel(const int* __restrict__ n_samples, int B, Geo
     if (tid == 255) s_run = run + s_scan[cur][255];
     __syncthreads();
   }
-}
-
-cudaError_t run_tile_prefix(const int* n_samples, int B, const Geometry& g, int TT, int T_cap,
-                            int* prefix, void* stream) {
-  return launch(tile_prefix_kernel, dim3(1), dim3(256), 0, stream, false, n_samples, B, g, TT, T_cap,
-                prefix);
 }
 
 template <int C, int TT>
@@ -352,8 +344,6 @@ __global__ void cov_finalize_kernel(const float* __restrict__ partials, int B, i
   }
 }
 
-cudaError_t run_bits_to_float(const unsigned* bits, int n, float* out, void* stream);
-
 template <int C>
 static cudaError_t run_cov_finalize_t(const float* partials, int B, int F, TileSched sched, int n_ctas,
                                       int slots, float2* Rs, float2* Rn, void* stream) {
@@ -361,8 +351,8 @@ static cudaError_t run_cov_finalize_t(const float* partials, int B, int F, TileS
   return launch(cov_finalize_kernel<C>, dim3((unsigned)((2 * n + 127) / 128)), dim3(128), 0, stream, true,
                 partials, B, F, sched, n_ctas, slots, Rs, Rn);
 }
-cudaError_t run_cov_finalize(int C, const float* partials, int B, int F, TileSched sched, int n_ctas,
-                             int slots, float2* Rs, float2* Rn, void* stream) {
+static cudaError_t run_cov_finalize(int C, const float* partials, int B, int F, TileSched sched, int n_ctas,
+                                    int slots, float2* Rs, float2* Rn, void* stream) {
   switch (C) {
     case 1: return run_cov_finalize_t<1>(partials, B, F, sched, n_ctas, slots, Rs, Rn, stream);
     case 2: return run_cov_finalize_t<2>(partials, B, F, sched, n_ctas, slots, Rs, Rn, stream);
@@ -378,18 +368,12 @@ static size_t stft_cov_smem_bytes(int hop) {
 }
 
 template <int C, int TT>
-static cudaError_t run_stft_cov_t(setk_plan* pl, StftCovArgs a, int B, int n_ctas, float2* Rs,
-                                  float2* Rn, float* maxabs, void* stream) {
+static cudaError_t run_stft_cov_t(const StftCovArgs& a, int n_ctas, void* stream) {
   const size_t smem = stft_cov_smem_bytes<C, TT>(a.g.hop);
   cudaError_t e = cudaFuncSetAttribute(stft_cov_kernel<C, TT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        (int)smem);
   if (e != cudaSuccess) return e;
-  e = launch(stft_cov_kernel<C, TT>, dim3(n_ctas), dim3(TT > 4 ? 320 : 288), smem, stream, false, a);
-  if (e != cudaSuccess) return e;
-  e = run_cov_finalize_t<C>(a.partials, B, a.g.F, a.sched, n_ctas, a.slots, Rs, Rn, stream);
-  if (e != cudaSuccess) return e;
-  if (maxabs) e = run_bits_to_float(a.maxabs_bits, B, maxabs, stream);
-  return e;
+  return launch(stft_cov_kernel<C, TT>, dim3(n_ctas), dim3(TT > 4 ? 320 : 288), smem, stream, false, a);
 }
 
 // Does a fused instantiation exist for this geometry?
@@ -401,7 +385,7 @@ bool stft_cov_fused_supported(const Geometry& g) {
 }
 
 // partial-sum workspace: floats per (utterance, chunk)
-size_t stft_cov_partial_floats(const Geometry& g) { return (size_t)(2 * g.C * g.C + 2) * g.F; }
+static size_t stft_cov_partial_floats(const Geometry& g) { return (size_t)(2 * g.C * g.C + 2) * g.F; }
 
 int stft_cov_pick_chunks(const setk_plan* pl, int B, int T) {
   // (chunk, utterance) grids of the workspace routes: all CTAs are equally long, so
@@ -423,66 +407,62 @@ int stft_cov_pick_chunks(const setk_plan* pl, int B, int T) {
   return best;
 }
 
-// CTA slots of the fused kernels (2 CTAs per SM resident: registers and shared memory)
-int fused_cta_slots(const setk_plan* pl) { return 2 * pl->sm_count; }
-
-// launch shape of the persistent schedule for a batch of B utterances of <= T frames
-void fused_schedule(const setk_plan* pl, int B, int T, int TT, int* n_ctas, int* slots, int* min_quota) {
-  const int G = fused_cta_slots(pl);
-  const int tiles_max = sched_tiles_of(T, TT);
+// The persistent schedule of a fused pass over B utterances of <= T frames, TT frames per tile and
+// at most T_cap frames of each used: the TileSched, the CTAs to launch and the partial-sum slots per
+// utterance.  A ragged batch (n_samples != null) keeps its lengths on the device, so this also
+// launches tile_prefix_kernel, which writes the tiles before every utterance to tile_prefix [B + 1].
+cudaError_t fused_schedule(const setk_plan* pl, int B, int T, int TT, int T_cap, const int* n_samples,
+                           int* tile_prefix, void* stream, TileSched* sched, int* n_ctas, int* slots) {
+  const int G = 2 * pl->sm_count;   // CTA slots: 2 CTAs per SM resident (registers and shared memory)
+  const int tiles_max = sched_tiles_of(imin(T, T_cap), TT);
   *slots = sched_slots(G, B);
-  *min_quota = sched_min_quota(tiles_max, *slots);
-  *n_ctas = sched_grid(B * tiles_max, G, *min_quota);
+  sched->prefix = n_samples ? tile_prefix : nullptr;
+  sched->tiles_u = tiles_max;
+  sched->B = B;
+  sched->min_quota = sched_min_quota(tiles_max, *slots);
+  *n_ctas = sched_grid(B * tiles_max, G, sched->min_quota);
+  if (!n_samples) return cudaSuccess;
+  return launch(tile_prefix_kernel, dim3(1), dim3(256), 0, stream, false, n_samples, B, pl->geo, TT, T_cap,
+                tile_prefix);
 }
 
-// frames per tile of the instantiation that serves C <= 3 channels (an odd C with TT = 5
-// would leave an odd number of half-warp jobs); the warp-specialised build for C = 4 also
-// uses 4 (stft_cov_ws_tt)
-static int sc_tt(int C) { return C == 2 ? kScTT : 4; }
+static const int kNoFrameCap = 0x7fffffff;
 
 size_t stft_cov_partial_bytes(const setk_plan* pl, int B, int T) {
-  int n_ctas, slots, mq;
-  fused_schedule(pl, B, T, sc_tt(pl->geo.C), &n_ctas, &slots, &mq);
+  TileSched sched;
+  int n_ctas, slots;
+  fused_schedule(pl, B, T, stft_cov_tt(pl->geo.C), kNoFrameCap, nullptr, nullptr, nullptr, &sched, &n_ctas,
+                 &slots);
   return sizeof(float) * stft_cov_partial_floats(pl->geo) * (size_t)slots * B;
 }
-
-bool stft_cov_ws_supported(const Geometry& g);
-cudaError_t run_stft_cov_ws(setk_plan*, const float*, const int*, int, int, int, const float*, const float*,
-                            unsigned, int*, float*, unsigned*, float2*, float2*, float*, void*);
 
 cudaError_t run_stft_cov_fused(setk_plan* pl, const float* audio, const int* n_samples, int B, int N,
                                int T, const float* mask_s, const float* mask_n, unsigned flags,
                                int* tile_prefix, float* partials, unsigned* maxabs_bits, float2* Rs,
                                float2* Rn, float* maxabs, void* stream) {
-  // C = 4: the warp-specialised build (stft_cov_ws.cu)
-  if (stft_cov_ws_supported(pl->geo))
-    return run_stft_cov_ws(pl, audio, n_samples, B, N, T, mask_s, mask_n, flags, tile_prefix, partials,
-                           maxabs_bits, Rs, Rn, maxabs, stream);
-  const int TT = sc_tt(pl->geo.C);
+  const Geometry& g = pl->geo;
   StftCovArgs a;
-  a.g = pl->geo;
+  a.g = g;
   a.audio = audio; a.n_samples = n_samples; a.N = N;
   a.mask_s = mask_s; a.mask_n = mask_n; a.flags = flags;
   a.T = T;
-  int n_ctas;
-  fused_schedule(pl, B, T, TT, &n_ctas, &a.slots, &a.sched.min_quota);
-  a.sched.B = B;
-  a.sched.tiles_u = sched_tiles_of(T, TT);
-  a.sched.prefix = nullptr;
-  if (n_samples) {     // ragged batch: the lengths live on the device
-    cudaError_t e = run_tile_prefix(n_samples, B, pl->geo, TT, 0x7fffffff, tile_prefix, stream);
-    if (e != cudaSuccess) return e;
-    a.sched.prefix = tile_prefix;
-  }
   a.window = pl->d_window;
   a.partials = partials;
   a.maxabs_bits = maxabs_bits;
-  switch (pl->geo.C) {
-    case 1: return run_stft_cov_t<1, 4>(pl, a, B, n_ctas, Rs, Rn, maxabs, stream);
-    case 2: return run_stft_cov_t<2, kScTT>(pl, a, B, n_ctas, Rs, Rn, maxabs, stream);
-    case 3: return run_stft_cov_t<3, 4>(pl, a, B, n_ctas, Rs, Rn, maxabs, stream);
+  int n_ctas;
+  cudaError_t e = fused_schedule(pl, B, T, stft_cov_tt(g.C), kNoFrameCap, n_samples, tile_prefix, stream,
+                                 &a.sched, &n_ctas, &a.slots);
+  if (e != cudaSuccess) return e;
+  switch (g.C) {
+    case 1: e = run_stft_cov_t<1, stft_cov_tt(1)>(a, n_ctas, stream); break;
+    case 2: e = run_stft_cov_t<2, stft_cov_tt(2)>(a, n_ctas, stream); break;
+    case 3: e = run_stft_cov_t<3, stft_cov_tt(3)>(a, n_ctas, stream); break;
+    case 4: e = run_stft_cov_ws(a, n_ctas, stream); break;   // the warp-specialised build (stft_cov_ws.cu)
     default: return cudaErrorInvalidValue;
   }
+  if (e == cudaSuccess) e = run_cov_finalize(g.C, partials, B, g.F, a.sched, n_ctas, a.slots, Rs, Rn, stream);
+  if (e == cudaSuccess && maxabs) e = run_bits_to_float(maxabs_bits, B, maxabs, stream);
+  return e;
 }
 
 }  // namespace setk

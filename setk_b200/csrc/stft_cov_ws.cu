@@ -42,6 +42,7 @@
 #include "common.cuh"
 #include "stft_tile.cuh"
 #include "stft_cov_args.cuh"
+#include "launchers.cuh"
 
 namespace setk {
 
@@ -533,61 +534,22 @@ __global__ void __maxnreg__(SETK_WS_LAUNCH_REGS) stft_cov_ws_kernel(StftCovArgs 
 }
 
 // ---- host side ----
-cudaError_t run_bits_to_float(const unsigned* bits, int n, float* out, void* stream);
-cudaError_t run_tile_prefix(const int* n_samples, int B, const Geometry& g, int TT, int T_cap,
-                            int* prefix, void* stream);
-cudaError_t run_cov_finalize(int C, const float* partials, int B, int F, TileSched sched, int n_ctas,
-                             int slots, float2* Rs, float2* Rn, void* stream);
-void fused_schedule(const setk_plan* pl, int B, int T, int TT, int* n_ctas, int* slots, int* min_quota);
-
-bool stft_cov_ws_supported(const Geometry& g) {
-  if (g.n_fft != 512 || g.C != 4) return false;
-  if (g.hop < 2 || g.hop > 512 || (g.hop & 1)) return false;
-  return true;
-}
-int stft_cov_ws_tt(int C) { return 16 / C; }
+static_assert(WsShape<4>::TT == stft_cov_tt(4),
+              "run_stft_cov_fused schedules the C = 4 launch in tiles of this kernel's TT frames");
 
 template <int C, bool HAS_MN>
-static cudaError_t run_ws_t(StftCovArgs a, int B, int n_ctas, float2* Rs, float2* Rn, float* maxabs,
-                            void* stream) {
+static cudaError_t run_ws_t(const StftCovArgs& a, int n_ctas, void* stream) {
   const size_t smem = WsSmem<C>::bytes(a.g.hop, HAS_MN ? 2 : 1);
   cudaError_t e = cudaFuncSetAttribute(stft_cov_ws_kernel<C, HAS_MN>,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  e = launch(stft_cov_ws_kernel<C, HAS_MN>, dim3(n_ctas), dim3(kWsThreads), smem, stream, false, a);
-  if (e != cudaSuccess) return e;
-  e = run_cov_finalize(C, a.partials, B, a.g.F, a.sched, n_ctas, a.slots, Rs, Rn, stream);
-  if (e != cudaSuccess) return e;
-  if (maxabs) e = run_bits_to_float(a.maxabs_bits, B, maxabs, stream);
-  return e;
+  return launch(stft_cov_ws_kernel<C, HAS_MN>, dim3(n_ctas), dim3(kWsThreads), smem, stream, false, a);
 }
 
-cudaError_t run_stft_cov_ws(setk_plan* pl, const float* audio, const int* n_samples, int B, int N, int T,
-                            const float* mask_s, const float* mask_n, unsigned flags, int* tile_prefix,
-                            float* partials, unsigned* maxabs_bits, float2* Rs, float2* Rn, float* maxabs,
-                            void* stream) {
-  const int TT = stft_cov_ws_tt(pl->geo.C);
-  StftCovArgs a;
-  a.g = pl->geo;
-  a.audio = audio; a.n_samples = n_samples; a.N = N;
-  a.mask_s = mask_s; a.mask_n = mask_n; a.flags = flags;
-  a.T = T;
-  int n_ctas;
-  fused_schedule(pl, B, T, TT, &n_ctas, &a.slots, &a.sched.min_quota);
-  a.sched.B = B;
-  a.sched.tiles_u = sched_tiles_of(T, TT);
-  a.sched.prefix = nullptr;
-  if (n_samples) {     // ragged batch: the lengths live on the device
-    cudaError_t e = run_tile_prefix(n_samples, B, pl->geo, TT, 0x7fffffff, tile_prefix, stream);
-    if (e != cudaSuccess) return e;
-    a.sched.prefix = tile_prefix;
-  }
-  a.window = pl->d_window;
-  a.partials = partials;
-  a.maxabs_bits = maxabs_bits;
-  if (pl->geo.C != 4) return cudaErrorInvalidValue;
-  if (mask_n) return run_ws_t<4, true>(a, B, n_ctas, Rs, Rn, maxabs, stream);
-  return run_ws_t<4, false>(a, B, n_ctas, Rs, Rn, maxabs, stream);
+// the C = 4 launch of the fused pass; run_stft_cov_fused prepares a and runs the finalize after it
+cudaError_t run_stft_cov_ws(const StftCovArgs& a, int n_ctas, void* stream) {
+  if (a.mask_n) return run_ws_t<4, true>(a, n_ctas, stream);
+  return run_ws_t<4, false>(a, n_ctas, stream);
 }
 
 }  // namespace setk

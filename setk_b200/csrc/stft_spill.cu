@@ -22,15 +22,14 @@
 #include "common.cuh"
 #include "stft_tile.cuh"
 #include "cov_spill_args.cuh"
+#include "launchers.cuh"
 
 namespace setk {
 
-// bins per (t, c) row in the workspace (float2 units): 264 for 257 bins, 520 for 513
-SETK_HD inline int spill_pitch(int n_fft) { return n_fft == 1024 ? 520 : 264; }
-constexpr int kSpillPitch = 264;
+constexpr int kSpillPitch = bin_pitch(kBins);
 constexpr int kNfft2 = 1024;       // the second tile size (BASELINE config 3)
 constexpr int kBins2 = 513;
-constexpr int kSpillPitch2 = 520;
+constexpr int kSpillPitch2 = bin_pitch(kBins2);
 
 struct StftSpillArgs {
   Geometry g;
@@ -472,10 +471,10 @@ bool stft_spill_supported(const Geometry& g) {
 }
 
 size_t stft_spill_bytes(const Geometry& g, int B, int T) {
-  return sizeof(float2) * (size_t)B * T * g.C * spill_pitch(g.n_fft);
+  return sizeof(float2) * (size_t)B * T * g.C * bin_pitch(g.F);
 }
 size_t apply_spill_bytes(const Geometry& g, int B, int T) {
-  return sizeof(float2) * (size_t)B * T * spill_pitch(g.n_fft);
+  return sizeof(float2) * (size_t)B * T * bin_pitch(g.F);
 }
 
 // channel groups [first_group, first_group + count) of CG channels each
@@ -483,7 +482,7 @@ template <int CG>
 static cudaError_t run_spill_t(StftSpillArgs a, int B, void* stream, int first_group, int count) {
   StftSpillArgs s = a;
   s.audio = a.audio + (long long)first_group * 4 * a.N;      // the kernels take c0 from blockIdx.y
-  s.xws = a.xws + (long long)first_group * 4 * spill_pitch(a.g.n_fft);
+  s.xws = a.xws + (long long)first_group * 4 * bin_pitch(a.g.F);
   if (a.g.n_fft == kNfft2) {
     const size_t smem = sizeof(float) * Tile1024<CG>::floats(a.g.hop);
     cudaError_t e = cudaFuncSetAttribute(stft_spill1024_kernel<CG>,
@@ -523,10 +522,6 @@ cudaError_t run_stft_spill(setk_plan* pl, const float* audio, const int* n_sampl
     default: return e;
   }
 }
-
-int stft_cov_pick_chunks(const setk_plan*, int, int);
-int cov_mma_bins_per_cta(int C);
-cudaError_t run_cov_mma(const CovSpillArgs& a, int B, void* stream);
 
 // C >= 5: the covariance is a real dense contraction (2C x 2C Gram blocks over T frames) and runs
 // on the tensor cores (cov_mma.cu); C <= 4 keeps the CUDA-core cov_spill_kernel
@@ -573,7 +568,7 @@ cudaError_t run_cov_spill(setk_plan* pl, const float2* xws, const float* mask_s,
                           unsigned flags, const int* n_samples, int B, int N, int T, int n_chunks,
                           float* partials, float2* Rs, float2* Rn, void* stream) {
   CovSpillArgs a;
-  a.xws = xws; a.pitch = spill_pitch(pl->geo.n_fft);
+  a.xws = xws; a.pitch = bin_pitch(pl->geo.F);
   a.mask_s = mask_s; a.mask_n = mask_n; a.flags = flags;
   a.n_samples = n_samples; a.N = N; a.g = pl->geo;
   a.T = T; a.F = pl->geo.F;
@@ -592,14 +587,14 @@ cudaError_t run_cov_spill(setk_plan* pl, const float2* xws, const float* mask_s,
 cudaError_t run_spill_to_bcft(const setk_plan* pl, const float2* xws, int B, int T, float2* out, void* stream) {
   const Geometry& g = pl->geo;
   return launch(spill_to_bcft_kernel, dim3((T + 31) / 32, (g.F + 31) / 32, B * g.C), dim3(256), 0, stream,
-                false, xws, spill_pitch(g.n_fft), g.C, g.F, T, out);
+                false, xws, bin_pitch(g.F), g.C, g.F, T, out);
 }
 
 // y = w^H x over the workspace -> yws [B][T][pitch]
 cudaError_t run_apply_spill(setk_plan* pl, const float2* xws, const void* w, int w_dtype,
                             const float* post_mask, int B, int T, float2* yws, void* stream) {
   ApplySpillArgs a;
-  a.xws = xws; a.pitch = spill_pitch(pl->geo.n_fft);
+  a.xws = xws; a.pitch = bin_pitch(pl->geo.F);
   a.w = w; a.w_dtype = w_dtype; a.post_mask = post_mask;
   a.C = pl->geo.C; a.F = pl->geo.F; a.T = T;
   const int nbb = (a.F + 287) / 288;

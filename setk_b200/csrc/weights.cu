@@ -10,6 +10,7 @@
 //   PmwfBeamformer.weight/_snr 620-659, GevdBeamformer.weight 674-682.
 #include "common.cuh"
 #include "hermitian_solve.cuh"
+#include "launchers.cuh"
 #include "weights_args.cuh"
 
 namespace setk {
@@ -248,9 +249,6 @@ __global__ void __launch_bounds__(128) pmwf_select_kernel(WeightsArgs a) {
   if (st) atomicOr(a.status + b, st);
 }
 
-bool weights_coop_supported(const WeightsArgs& a, int C);
-cudaError_t weights_coop_launch(const WeightsArgs& a, int C, void* stream);
-
 template <int C>
 static cudaError_t launch_weights(const WeightsArgs& a, void* stream) {
   if (weights_coop_supported(a, C)) return weights_coop_launch(a, C, stream);
@@ -270,7 +268,7 @@ static cudaError_t launch_weights(const WeightsArgs& a, void* stream) {
   return e;
 }
 
-cudaError_t weights_dispatch(const WeightsArgs& a, int C, void* stream) {
+static cudaError_t weights_dispatch(const WeightsArgs& a, int C, void* stream) {
   switch (C) {
 #define SETK_CASE(n) case n: return launch_weights<n>(a, stream);
     SETK_CASE(1) SETK_CASE(2) SETK_CASE(3) SETK_CASE(4) SETK_CASE(5) SETK_CASE(6) SETK_CASE(7) SETK_CASE(8)
@@ -281,7 +279,7 @@ cudaError_t weights_dispatch(const WeightsArgs& a, int C, void* stream) {
 }
 
 // Scratch of the PMWF automatic reference selection: allocated per call on the caller's
-// stream (cudaMallocAsync / cudaFreeAsync, like wpe_entry and setk_cgmm_stft), so calls on
+// stream (cudaMallocAsync / cudaFreeAsync, like the plan-free entry points of api.cu), so calls on
 // different streams or devices never share it.
 cudaError_t weights_run(int kind, double beta, int ref_channel, int rank1, int ban, const void* Rs,
                         const void* Rn, const void* Ry, int r_dtype, int B, int F, int C, void* w,

@@ -11,6 +11,7 @@
 // Kinds: MVDR (beamformer.py:527-539), MPDR (555-573), GEVD / PEVD (31-63, 674-682), with BAN
 // (14-28).  MPDR-whiten, PMWF and the rank-1 options stay on weights.cu.
 #include "jacobi_coop.cuh"
+#include "launchers.cuh"
 #include "lu_coop.cuh"
 #include "weights_args.cuh"
 

@@ -6,6 +6,7 @@
 // (inside the weight solve both are applied in registers by weights.cu).
 #include "common.cuh"
 #include "hermitian_solve.cuh"
+#include "launchers.cuh"
 
 namespace setk {
 

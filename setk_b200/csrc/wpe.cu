@@ -23,6 +23,7 @@
 #include <cstdlib>
 #include "common.cuh"
 #include "hermitian_solve.cuh"
+#include "launchers.cuh"
 
 namespace setk {
 

@@ -9,12 +9,15 @@ OUT="$HERE/libsetk_b200_emu.so"
 OBJ="$HERE/obj"
 mkdir -p "$OBJ"
 pids=()
-for f in api generic weights weights_coop weights_post stft_cov_fused stft_cov_ws apply_istft_fused stft_spill cov_mma cgmm wpe spatial cm_mask; do
-  g++ -O2 -std=c++17 -DSETK_EMU -DSETK_TABLE_CHUNK=8 -fPIC -pthread -I"$HERE" -I"$ROOT/include" -x c++ -c "$SRC/$f.cu" -o "$OBJ/$f.o" &
+objs=("$OBJ/cuda_emu.o")
+for src in "$SRC"/*.cu; do
+  o="$OBJ/$(basename "$src" .cu).o"
+  objs+=("$o")
+  g++ -O2 -std=c++17 -DSETK_EMU -DSETK_TABLE_CHUNK=8 -fPIC -pthread -I"$HERE" -I"$ROOT/include" -x c++ -c "$src" -o "$o" &
   pids+=($!)
 done
 g++ -O2 -std=c++17 -DSETK_EMU -fPIC -pthread -I"$HERE" -c "$HERE/cuda_emu.cc" -o "$OBJ/cuda_emu.o" &
 pids+=($!)
 for p in "${pids[@]}"; do wait $p; done
-g++ -shared -pthread -o "$OUT" "$OBJ"/*.o
+g++ -shared -pthread -o "$OUT" "${objs[@]}"
 echo "built $OUT"

@@ -1,6 +1,7 @@
 """
 CPU tier: the balanced persistent schedule of the fused kernels (TileSched, sched_* in
-setk_b200/csrc/stft_tile.cuh; fused_schedule in stft_cov_fused.cu), restated in Python and
+setk_b200/csrc/stft_tile.cuh; fused_schedule in stft_cov_fused.cu, which sets it up for the
+fused STFT + covariance and the fused apply + iSTFT alike), restated in Python and
 checked over random batch shapes: every (utterance, tile) pair is owned by exactly one CTA,
 a CTA's partial-sum slot index stays below the reserved slot count, and cov_finalize_kernel's
 "slots used by utterance b" formula names exactly the slots that were written.
