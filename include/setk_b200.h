@@ -6,7 +6,8 @@
  *   PMWF weight solve (+BAN, rank-1) -> beamform apply -> iSTFT (+peak norm)
  *
  * and the front ends around it: CGMM masks, WPE / WPD, spatial features, sound
- * source localisation and AuxIVA blind source separation.
+ * source localisation, AuxIVA blind source separation and iMCRA / OM-LSA
+ * noise suppression.
  *
  * Every entry point below replaces one reference interface; the citation is
  * the reference file:line (paths relative to the reference tree).  The Python
@@ -371,6 +372,41 @@ int setk_ssl(int32_t backend, const void* stft, int32_t B, int32_t M, int32_t F,
  */
 int setk_auxiva_stft(const void* stft, int32_t B, int32_t N, int32_t F, int32_t T, int32_t num_epochs,
                      void* out, uint32_t* status, void* stream);
+
+/* ---- single-channel noise suppression: scripts/sptk/libs/ns.py iMCRA, apply_ns.py ---- */
+#define SETK_NS_MAX_W 8         /* w_mcra <= 8: at most 17 smoothing taps */
+#define SETK_NS_MAX_U 64        /* U <= 64 frames of sub-window minima */
+#define SETK_NS_MAX_BINS 2049   /* F <= 2049 (n_fft 4096) */
+
+typedef struct setk_imcra_config {   /* iMCRA.__init__ keywords, ns.py:221-245, and run(eps), ns.py:247 */
+  double alpha, alpha_s, alpha_d, b_min, gamma0, gamma1, zeta0, xi_min_db, gmin_db, beta, eps;
+  int32_t w_mcra, V, U, reserved;
+  const double* window_host;         /* HOST pointer, 2*w_mcra+1 values of
+                                        scipy.signal.get_window(h_mcra, 2*w_mcra+1) (ns.py:243) */
+} setk_imcra_config_t;
+
+/*
+ * iMCRA noise estimation + OM-LSA gain: iMCRA(**cfg).run(stft, eps) (ns.py:247-387) for every
+ * utterance of the batch; apply_ns.py:41-42 multiplies the gain into the STFT.  Plan-free; scratch (only
+ * when U > V) is stream-ordered.  fp64 after the complex64 input.
+ *   stft      c64 [B][F][T]   (the reference's T x F per utterance, bins before frames here: what a
+ *                              one-channel setk_stft writes)
+ *   n_frames  i32 [B] or NULL (= T): utterance b runs over its first n_frames[b] frames; later frames
+ *                              get gain 0 and enh 0
+ *   gain      f64 [B][T][F] or NULL   the reference's T x F gain (ns.py:383-387)
+ *   enh       c64 [B][F][T] or NULL   gain * stft (apply_ns.py:42), ready for setk_istft
+ * Per frame (ns.py line by line): lambda_d = beta lambda_d_hat (269); gamma (272, NOT floored); xi_hat
+ * (275-280); v, gh1 = xi/(1+xi) exp(E1(v)/2) (283-284); var_sf = conv(|x|^2, w_m, "same") (288);
+ * var_s and its minima (291-301); indicator (304-307); var_sf_hat from the previous var_s_hat (311-317);
+ * var_s_hat and its minima (320-329); q_hat, p_hat (332-358); lambda_d_hat (362-367); every V frames
+ * the minima over the last U per-frame sub-window minima (370-380); gain = gh1^p gmin^(1-p) (383).
+ * E1(0) is the 37.191280375549404 the reference's quad returns there, not +inf.
+ * SETK_EINVAL: a null cfg, window or stft; gain and enh both NULL; B, F or T < 1;
+ * F > SETK_NS_MAX_BINS; w_mcra outside [0, SETK_NS_MAX_W]; F < 2*w_mcra+1 (np.convolve would swap
+ * its operands, ns.py:288); V < 1; U outside [1, SETK_NS_MAX_U].
+ */
+int setk_ns_imcra(const setk_imcra_config_t* cfg, const void* stft, const int32_t* n_frames, int32_t B,
+                  int32_t F, int32_t T, double* gain, void* enh, void* stream);
 
 /* floor(y * 32768) clipped to int16: the PCM_16 conversion of
  * WaveWriter.write -> write_wav -> soundfile (data_handler.py:600-605,

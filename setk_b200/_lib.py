@@ -30,6 +30,7 @@ F_CLIP_MASK, F_MASK_FT = 1, 2
 C64, C128 = 0, 1
 SSL_ML, SSL_SRP, SSL_MUSIC = 0, 1, 2
 SSL_MAX_MASKS = 8
+NS_MAX_W, NS_MAX_U, NS_MAX_BINS = 8, 64, 2049
 
 
 class SetkConfig(Structure):
@@ -37,6 +38,14 @@ class SetkConfig(Structure):
                 ("n_fft", c_int32), ("frame_hop", c_int32),
                 ("center", c_int32), ("max_batch", c_int32),
                 ("max_samples", c_int32), ("reserved", c_int32),
+                ("window_host", POINTER(c_double))]
+
+
+class ImcraConfig(Structure):
+    _fields_ = [("alpha", c_double), ("alpha_s", c_double), ("alpha_d", c_double), ("b_min", c_double),
+                ("gamma0", c_double), ("gamma1", c_double), ("zeta0", c_double), ("xi_min_db", c_double),
+                ("gmin_db", c_double), ("beta", c_double), ("eps", c_double),
+                ("w_mcra", c_int32), ("V", c_int32), ("U", c_int32), ("reserved", c_int32),
                 ("window_host", POINTER(c_double))]
 
 
@@ -108,6 +117,8 @@ _PROTOTYPES = {
                          c_void_p, c_void_p, c_void_p]),
     "setk_auxiva_stft": (c_int, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p,
                                  c_void_p]),
+    "setk_ns_imcra": (c_int, [POINTER(ImcraConfig), c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p,
+                              c_void_p, c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)

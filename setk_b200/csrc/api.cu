@@ -650,4 +650,30 @@ int setk_auxiva_stft(const void* stft, int32_t B, int32_t N, int32_t F, int32_t 
   });
 }
 
+// ---- iMCRA / OM-LSA noise suppression (ns.cu) ----
+int setk_ns_imcra(const setk_imcra_config_t* cfg, const void* stft, const int32_t* n_frames, int32_t B,
+                  int32_t F, int32_t T, double* gain, void* enh, void* stream) {
+  if (!cfg || !cfg->window_host || !stft) return fail(SETK_EINVAL, "setk_ns_imcra: null argument");
+  if (!gain && !enh) return fail(SETK_EINVAL, "setk_ns_imcra: gain and enh are both null");
+  if (B < 1 || F < 1 || T < 1 || F > SETK_NS_MAX_BINS || B > 65535)
+    return fail(SETK_EINVAL, "setk_ns_imcra: bad shape B=%d F=%d T=%d (F <= %d)", B, F, T, SETK_NS_MAX_BINS);
+  if (cfg->w_mcra < 0 || cfg->w_mcra > SETK_NS_MAX_W)
+    return fail(SETK_EINVAL, "setk_ns_imcra: w_mcra=%d outside [0, %d]", cfg->w_mcra, SETK_NS_MAX_W);
+  if (F < 2 * cfg->w_mcra + 1)
+    return fail(SETK_EINVAL, "setk_ns_imcra: F=%d bins < %d smoothing taps", F, 2 * cfg->w_mcra + 1);
+  if (cfg->V < 1) return fail(SETK_EINVAL, "setk_ns_imcra: V=%d < 1", cfg->V);
+  if (cfg->U < 1 || cfg->U > SETK_NS_MAX_U)
+    return fail(SETK_EINVAL, "setk_ns_imcra: U=%d outside [1, %d]", cfg->U, SETK_NS_MAX_U);
+  const float2* X = static_cast<const float2*>(stft);
+  float2* out = static_cast<float2*>(enh);
+  const size_t ring = ns_ring_bytes(*cfg, B, F);
+  if (ring == 0) {
+    cudaError_t e = run_ns_imcra(*cfg, X, n_frames, B, F, T, nullptr, gain, out, stream);
+    return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_ns_imcra");
+  }
+  return with_scratch(ring, stream, "setk_ns_imcra(workspace)", "setk_ns_imcra", [&](char* ws) {
+    return run_ns_imcra(*cfg, X, n_frames, B, F, T, reinterpret_cast<double*>(ws), gain, out, stream);
+  });
+}
+
 }  // extern "C"

@@ -116,6 +116,11 @@ cudaError_t run_ssl(int backend, const float2* stft, int B, int M, int F, int T,
                     double compression, double eps, int normalize, char* ws, double* scores, int* index,
                     void* stream);
 
+// ---- ns.cu: iMCRA noise estimation and the OM-LSA gain ----
+size_t ns_ring_bytes(const setk_imcra_config_t& cfg, int B, int F);
+cudaError_t run_ns_imcra(const setk_imcra_config_t& cfg, const float2* X, const int* n_frames, int B, int F,
+                         int T, double* ring, double* gain, float2* enh, void* stream);
+
 // ---- cm_mask.cu: Kaldi compressed-matrix masks ----
 cudaError_t run_cm_masks(const unsigned char* blobs, long long slot_bytes, int B, int T, int F, float* out,
                          int* status, void* stream);

@@ -620,3 +620,59 @@ def auxiva_from_stft(stft, num_epochs=20):
             _lib.ptr(stft), B, N, F, T, int(num_epochs), _lib.ptr(out), _lib.ptr(status),
             _lib.current_stream(stft.device)))
     return out, status
+
+
+# ---------------------------------------------------------------------------
+# iMCRA / OM-LSA noise suppression on explicit STFTs (libs/ns.py, apply_ns.py of the reference; csrc/ns.cu)
+# ---------------------------------------------------------------------------
+IMCRA_DEFAULTS = dict(alpha=0.92, alpha_s=0.9, alpha_d=0.85, b_min=1.66, gamma0=4.6, gamma1=3, zeta0=1.67,
+                      xi_min_db=-18, gmin_db=-10, w_mcra=1, h_mcra="hann", beta=1.47, V=15, U=8)
+
+
+def imcra_config(config=None, eps=1e-7):
+    """
+    setk_imcra_config_t from iMCRA keywords (ns.py:221-245; missing ones take the reference's
+    defaults) and run(eps).  Returns (config, window): keep `window` alive while the config is used.
+    """
+    conf = dict(IMCRA_DEFAULTS, **(config or {}))
+    unknown = set(conf) - set(IMCRA_DEFAULTS)
+    if unknown:
+        raise TypeError(f"unknown iMCRA keywords: {sorted(unknown)}")
+    w_mcra = int(conf["w_mcra"])
+    if w_mcra < 0 or w_mcra > _lib.NS_MAX_W:
+        raise ValueError(f"w_mcra={w_mcra} outside [0, {_lib.NS_MAX_W}]")
+    window = np.ascontiguousarray(scipy.signal.get_window(conf["h_mcra"], 2 * w_mcra + 1), dtype=np.float64)
+    cfg = _lib.ImcraConfig(
+        alpha=conf["alpha"], alpha_s=conf["alpha_s"], alpha_d=conf["alpha_d"], b_min=conf["b_min"],
+        gamma0=conf["gamma0"], gamma1=conf["gamma1"], zeta0=conf["zeta0"], xi_min_db=conf["xi_min_db"],
+        gmin_db=conf["gmin_db"], beta=conf["beta"], eps=float(eps), w_mcra=w_mcra, V=int(conf["V"]),
+        U=int(conf["U"]), reserved=0, window_host=window.ctypes.data_as(ctypes.POINTER(ctypes.c_double)))
+    return cfg, window
+
+
+def ns_from_stft(stft, n_frames=None, config=None, gain=True, enh=True, eps=1e-7):
+    """
+    iMCRA(**config).run(stft, eps) batched (ns.py:247-387), and gain * stft (apply_ns.py:42).
+    stft (B,F,T) complex64; n_frames (B,) int or None (every utterance has T frames).
+    Returns (gain (B,T,F) float64 or None, enh (B,F,T) complex64 or None).
+    """
+    stft = _c64(stft)
+    if stft.dim() != 3:
+        raise ValueError(f"stft must be (B, F, T), got {tuple(stft.shape)}")
+    if not (gain or enh):
+        raise ValueError("ns_from_stft: ask for the gain, the enhanced STFT or both")
+    B, F, T = stft.shape
+    dev = stft.device
+    nf = None
+    if n_frames is not None:
+        nf = torch.as_tensor(n_frames, device=dev).to(torch.int32).contiguous()
+        if nf.shape != (B,):
+            raise ValueError(f"n_frames must have shape ({B},)")
+    g = torch.empty((B, T, F), dtype=torch.float64, device=dev) if gain else None
+    e = torch.empty((B, F, T), dtype=torch.complex64, device=dev) if enh else None
+    cfg, window = imcra_config(config, eps)
+    with _ctx(dev):
+        _lib.check(_lib.library().setk_ns_imcra(ctypes.byref(cfg), _lib.ptr(stft), _lib.ptr(nf), B, F, T,
+                                                _lib.ptr(g), _lib.ptr(e), _lib.current_stream(dev)))
+    del window
+    return g, e
