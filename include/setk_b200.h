@@ -6,8 +6,8 @@
  *   PMWF weight solve (+BAN, rank-1) -> beamform apply -> iSTFT (+peak norm)
  *
  * and the front ends around it: CGMM masks, WPE / WPD, spatial features, sound
- * source localisation, AuxIVA blind source separation and iMCRA / OM-LSA
- * noise suppression.
+ * source localisation, AuxIVA blind source separation, iMCRA / OM-LSA
+ * noise suppression and image-method room impulse responses.
  *
  * Every entry point below replaces one reference interface; the citation is
  * the reference file:line (paths relative to the reference tree).  The Python
@@ -19,7 +19,8 @@
  *   - all data pointers are DEVICE pointers unless the name ends in _host;
  *   - every call is asynchronous on the caller's `stream` (a cudaStream_t passed
  *     as void*), re-entrant, and keeps no global state besides the last error
- *     string (thread local);
+ *     string (thread local); setk_rir_image alone synchronises its stream (it
+ *     reads the room sizes back to size the launch);
  *   - arrays are dense, row-major, the reference's axis order:
  *       audio  f32 [B][C][N]          (read_wav: C x N, utils.py:65-92)
  *       mask   f32 [B][T][F]          (T x F, beamformer.py:89)
@@ -407,6 +408,52 @@ typedef struct setk_imcra_config {   /* iMCRA.__init__ keywords, ns.py:221-245, 
  */
 int setk_ns_imcra(const setk_imcra_config_t* cfg, const void* stft, const int32_t* n_frames, int32_t B,
                   int32_t F, int32_t T, double* gain, void* enh, void* stream);
+
+/* ---- room impulse responses: include/rir-generator.{h,cc} (rir-simulate), rir_generate_{1d,2d}.py ---- */
+#define SETK_MIC_OMNI 0                /* rho = 1     rir-generator.cc:196-212 */
+#define SETK_MIC_SUBCARDIOID 1         /* rho = 0.75 */
+#define SETK_MIC_CARDIOID 2            /* rho = 0.5  */
+#define SETK_MIC_HYPERCARDIOID 3       /* rho = 0.25 */
+#define SETK_MIC_BIDIRECTIONAL 4       /* rho = 0    */
+#define SETK_RIR_MAX_TW 512            /* window taps Tw <= 512: fs < 64125 Hz */
+#define SETK_RIR_MAX_HALF 2048         /* lattice half-width n = ceil(L / (2 T)) <= 2048 per axis */
+#define SETK_RIR_MAX_CANDIDATES 4294967296.0   /* 8 (2nx+1)(2ny+1)(2nz+1) <= 2^32 images per channel */
+
+typedef struct setk_rir_config {
+  double sound_velocity, samp_frequency;         /* c, fs; both >= 1 (rir-generator.cc:29-30) */
+  double azimuth, elevation;                     /* receiver orientation, radians (only for non-omni) */
+  int32_t n_samples, order, mic_type, hp_filter; /* L >= 1; order >= -1 (-1: every order); SETK_MIC_* */
+} setk_rir_config_t;
+
+/*
+ * Image-method room impulse responses: RirGenerator::GenerateRir (rir-generator.cc:108-192, with
+ * MicrophoneSim 194-223 and Sinc, rir-generator.h:156) for B problems b = (room, beta, source), each
+ * with M receivers.  Plan-free; scratch (several segments with the filter) is stream-ordered.  The
+ * call reads `room` back to the host to check it and size the launch, so it synchronises `stream`.
+ *   room       f64 [B][3]     room dimensions, metres
+ *   beta       f64 [B][6]     reflection coefficients of the walls x=0, x=Lx, y=0, y=Ly, z=0, z=Lz
+ *                             (a T60 becomes these on the host: setk_b200.plan.rir_beta,
+ *                             rir-generator.cc:78-92)
+ *   source     f64 [B][3]     metres
+ *   receivers  f64 [B][M][3]  metres
+ *   rir        f32 [B][M][L]  the response, written whole
+ *   status     u32 [B] or NULL  SETK_ST_NONFINITE when a tap is not finite or |tap| >= 4096, or a
+ *                             sample leaves the accumulator's range (caller zeroes it)
+ * Per image (x, y, z in [-n, n], q, j, k in {0, 1}): distance in samples from (1-2q)S - R + 2xT,
+ * reflection factor beta0^|x-q| beta1^|x| beta2^|y-j| beta3^|y| beta4^|z-k| beta5^|z|, kept when
+ * |2x-q| + |2y-j| + |2z-k| <= order (or order == -1) and floor(dist) < L; Tw = 2 int(0.004 fs + 0.5)
+ * Hann-windowed sinc taps from floor(dist) - Tw/2 + 1, gain mic * refl / (4 pi dist c/fs), taps
+ * outside [0, L) dropped; then the 100 Hz high-pass (180-190) when hp_filter != 0.
+ * Differences from the reference: distances, floor and frac are fp64 (the reference's float32
+ * geometry is most of its own error), taps float32, the sum 64-bit fixed point (2^-44 per unit) so
+ * two calls are bit-identical, the high-pass fp64.
+ * SETK_EINVAL: a null pointer; B, M or L < 1; B or M > 65535; c or fs < 1; order < -1; an unknown
+ * mic_type; a room dimension <= 0 (the reference divides by it).
+ * SETK_EUNSUPPORTED: Tw > SETK_RIR_MAX_TW; a lattice half-width > SETK_RIR_MAX_HALF; more than
+ * SETK_RIR_MAX_CANDIDATES images per channel (a 1 m cube at 16 kHz reaches it at L = 38 119, 2.4 s).
+ */
+int setk_rir_image(const setk_rir_config_t* cfg, const double* room, const double* beta, const double* source,
+                   const double* receivers, int32_t B, int32_t M, float* rir, uint32_t* status, void* stream);
 
 /* floor(y * 32768) clipped to int16: the PCM_16 conversion of
  * WaveWriter.write -> write_wav -> soundfile (data_handler.py:600-605,

@@ -31,6 +31,7 @@ C64, C128 = 0, 1
 SSL_ML, SSL_SRP, SSL_MUSIC = 0, 1, 2
 SSL_MAX_MASKS = 8
 NS_MAX_W, NS_MAX_U, NS_MAX_BINS = 8, 64, 2049
+MIC_TYPES = ("omnidirectional", "subcardioid", "cardioid", "hypercardioid", "bidirectional")  # SETK_MIC_*
 
 
 class SetkConfig(Structure):
@@ -47,6 +48,12 @@ class ImcraConfig(Structure):
                 ("gmin_db", c_double), ("beta", c_double), ("eps", c_double),
                 ("w_mcra", c_int32), ("V", c_int32), ("U", c_int32), ("reserved", c_int32),
                 ("window_host", POINTER(c_double))]
+
+
+class RirConfig(Structure):
+    _fields_ = [("sound_velocity", c_double), ("samp_frequency", c_double), ("azimuth", c_double),
+                ("elevation", c_double), ("n_samples", c_int32), ("order", c_int32), ("mic_type", c_int32),
+                ("hp_filter", c_int32)]
 
 
 class SetkError(RuntimeError):
@@ -119,6 +126,8 @@ _PROTOTYPES = {
                                  c_void_p]),
     "setk_ns_imcra": (c_int, [POINTER(ImcraConfig), c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p,
                               c_void_p, c_void_p]),
+    "setk_rir_image": (c_int, [POINTER(RirConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32,
+                               c_void_p, c_void_p, c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)

@@ -676,4 +676,55 @@ int setk_ns_imcra(const setk_imcra_config_t* cfg, const void* stft, const int32_
   });
 }
 
+// ---- image-method room impulse responses (rir.cu) ----
+int setk_rir_image(const setk_rir_config_t* cfg, const double* room, const double* beta, const double* source,
+                   const double* receivers, int32_t B, int32_t M, float* rir, uint32_t* status, void* stream) {
+  if (!cfg || !room || !beta || !source || !receivers || !rir) return fail(SETK_EINVAL, "setk_rir_image: null argument");
+  const int L = cfg->n_samples;
+  if (B < 1 || M < 1 || L < 1 || B > 65535 || M > 65535)
+    return fail(SETK_EINVAL, "setk_rir_image: bad shape B=%d M=%d L=%d", B, M, L);
+  if (!(cfg->sound_velocity >= 1) || !(cfg->samp_frequency >= 1))
+    return fail(SETK_EINVAL, "setk_rir_image: c=%g and fs=%g must be >= 1", cfg->sound_velocity, cfg->samp_frequency);
+  if (cfg->order < -1) return fail(SETK_EINVAL, "setk_rir_image: order=%d < -1", cfg->order);
+  if (cfg->mic_type < SETK_MIC_OMNI || cfg->mic_type > SETK_MIC_BIDIRECTIONAL)
+    return fail(SETK_EINVAL, "setk_rir_image: unknown mic_type %d", cfg->mic_type);
+  const int Tw = rir_window_taps(cfg->samp_frequency);
+  if (Tw > SETK_RIR_MAX_TW)
+    return fail(SETK_EUNSUPPORTED, "setk_rir_image: fs=%g gives Tw=%d > %d taps", cfg->samp_frequency, Tw,
+                SETK_RIR_MAX_TW);
+  std::vector<double> dims((size_t)B * 3);
+  cudaError_t e = cudaMemcpyAsync(dims.data(), room, sizeof(double) * dims.size(), cudaMemcpyDeviceToHost,
+                                  static_cast<cudaStream_t>(stream));
+  if (e == cudaSuccess) e = cudaStreamSynchronize(static_cast<cudaStream_t>(stream));
+  if (e != cudaSuccess) return cuda_fail(e, "setk_rir_image(room)");
+  const double cts = cfg->sound_velocity / cfg->samp_frequency;
+  int max_n = 0;
+  for (int b = 0; b < B; ++b) {
+    double cand = 8;
+    for (int d = 0; d < 3; ++d) {
+      const double r = dims[(size_t)b * 3 + d];
+      if (!(r > 0) || !std::isfinite(r))
+        return fail(SETK_EINVAL, "setk_rir_image: problem %d: room dimension %d is %g, not > 0", b, d, r);
+      const double n = rir_lattice_half(L, r, cts);
+      if (n > SETK_RIR_MAX_HALF)
+        return fail(SETK_EUNSUPPORTED, "setk_rir_image: problem %d: lattice half-width %.0f > %d along axis %d",
+                    b, n, SETK_RIR_MAX_HALF, d);
+      max_n = imax(max_n, (int)n);
+      cand *= 2 * n + 1;
+    }
+    if (cand > SETK_RIR_MAX_CANDIDATES)
+      return fail(SETK_EUNSUPPORTED, "setk_rir_image: problem %d: %.3g images per channel > %.3g", b, cand,
+                  SETK_RIR_MAX_CANDIDATES);
+  }
+  if (rir_segments(L) == 1 || !cfg->hp_filter) {
+    e = run_rir_image(*cfg, room, beta, source, receivers, B, M, max_n, rir, nullptr, status, stream);
+    return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_rir_image");
+  }
+  return with_scratch(sizeof(double) * (size_t)B * M * L, stream, "setk_rir_image(workspace)", "setk_rir_image",
+                      [&](char* ws) {
+    return run_rir_image(*cfg, room, beta, source, receivers, B, M, max_n, rir, reinterpret_cast<double*>(ws),
+                         status, stream);
+  });
+}
+
 }  // extern "C"

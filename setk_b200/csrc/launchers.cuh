@@ -121,6 +121,14 @@ size_t ns_ring_bytes(const setk_imcra_config_t& cfg, int B, int F);
 cudaError_t run_ns_imcra(const setk_imcra_config_t& cfg, const float2* X, const int* n_frames, int B, int F,
                          int T, double* ring, double* gain, float2* enh, void* stream);
 
+// ---- rir.cu: image-method room impulse responses ----
+double rir_lattice_half(int L, double room, double cts);
+int rir_window_taps(double fs);
+int rir_segments(int L);
+cudaError_t run_rir_image(const setk_rir_config_t& cfg, const double* room, const double* beta,
+                          const double* source, const double* receivers, int B, int M, int max_n, float* rir,
+                          double* ws, unsigned* status, void* stream);
+
 // ---- cm_mask.cu: Kaldi compressed-matrix masks ----
 cudaError_t run_cm_masks(const unsigned char* blobs, long long slot_bytes, int B, int T, int F, float* out,
                          int* status, void* stream);

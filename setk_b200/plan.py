@@ -676,3 +676,75 @@ def ns_from_stft(stft, n_frames=None, config=None, gain=True, enh=True, eps=1e-7
                                                 _lib.ptr(g), _lib.ptr(e), _lib.current_stream(dev)))
     del window
     return g, e
+
+
+# ---------------------------------------------------------------------------
+# Image-method room impulse responses (include/rir-generator.cc, rir_generate_{1d,2d}.py; csrc/rir.cu)
+# ---------------------------------------------------------------------------
+def rir_beta(room, rt60_or_refl, c=340):
+    """
+    Reflection coefficients (6,) float64 for one room: six coefficients pass through; one T60 (a
+    number or a one-element sequence) becomes sqrt(1 - alpha) on every wall, alpha = 24 V ln10 /
+    (c S T60), and T60 = 0 gives 0 (rir-generator.cc:78-92, in float64).  ValueError when alpha > 1.
+    """
+    refl = np.atleast_1d(np.asarray(rt60_or_refl, dtype=np.float64))
+    if refl.shape == (6,):
+        return refl.copy()
+    if refl.shape != (1,):
+        raise ValueError(f"beta must be one T60 or six reflection coefficients, got {refl.shape[0]} values")
+    t60 = float(refl[0])
+    lx, ly, lz = (float(v) for v in np.asarray(room, dtype=np.float64).reshape(3))
+    if t60 == 0:
+        return np.zeros(6)
+    V, S = lx * ly * lz, 2 * (lx * ly + lx * lz + ly * lz)
+    alpha = 24 * V * math.log(10.0) / (c * S * t60)
+    if alpha > 1:
+        raise ValueError(f"{alpha} > 1: The reflection coefficients cannot be calculated using the current "
+                         "room parameters, i.e. room size and reverberation time.")
+    return np.full(6, math.sqrt(1 - alpha))
+
+
+def rir_image(room, beta, source, receivers, n_samples, sr=16000, c=340, order=-1, mic_type="omnidirectional",
+              orientation=(0, 0), hp_filter=True, device=None):
+    """
+    Image-method RIRs (rir-generator.cc:108-223) for B problems b = (room, beta, source) with M
+    receivers each: room (B,3), beta (B,6) reflection coefficients (rir_beta turns a T60 into them),
+    source (B,3), receivers (B,M,3), all metres; one problem may drop the leading B.  Returns
+    (B, M, n_samples) float32 on `device` (default: the inputs' device, else cuda).  A problem whose
+    response leaves the accumulator's range raises ValueError naming it.
+    """
+    if mic_type not in _lib.MIC_TYPES:
+        raise ValueError(f"unknown mic_type {mic_type!r}: one of {_lib.MIC_TYPES}")
+    if device is None:
+        device = next((t.device for t in (room, beta, source, receivers) if isinstance(t, torch.Tensor)),
+                      "cuda" if torch.cuda.is_available() else "cpu")
+    dev = torch.device(device)
+
+    def f64(t, shape):
+        t = torch.as_tensor(t, dtype=torch.float64, device=dev).contiguous()
+        return t.reshape(shape) if t.dim() == len(shape) - 1 else t
+
+    room = f64(room, (1, 3))
+    B = room.shape[0]
+    beta, source, receivers = f64(beta, (1, 6)), f64(source, (1, 3)), f64(receivers, (1, -1, 3))
+    if room.shape != (B, 3) or beta.shape != (B, 6) or source.shape != (B, 3) or receivers.dim() != 3 \
+            or receivers.shape[0] != B or receivers.shape[2] != 3:
+        raise ValueError(f"shapes room {tuple(room.shape)}, beta {tuple(beta.shape)}, source "
+                         f"{tuple(source.shape)}, receivers {tuple(receivers.shape)}: want (B,3), (B,6), "
+                         "(B,3), (B,M,3)")
+    M, L = receivers.shape[1], int(n_samples)
+    out = torch.empty((B, M, max(L, 0)), dtype=torch.float32, device=dev)
+    status = torch.zeros(B, dtype=torch.int32, device=dev)
+    az, el = (float(v) for v in orientation)
+    cfg = _lib.RirConfig(sound_velocity=float(c), samp_frequency=float(sr), azimuth=az, elevation=el,
+                         n_samples=L, order=int(order), mic_type=_lib.MIC_TYPES.index(mic_type),
+                         hp_filter=int(bool(hp_filter)))
+    with _ctx(dev):
+        _lib.check(_lib.library().setk_rir_image(ctypes.byref(cfg), _lib.ptr(room), _lib.ptr(beta),
+                                                 _lib.ptr(source), _lib.ptr(receivers), B, M, _lib.ptr(out),
+                                                 _lib.ptr(status), _lib.current_stream(dev)))
+    bad = torch.nonzero(status).flatten().tolist()
+    if bad:
+        raise ValueError(f"rir_image: the response of problem {bad[0]} is not finite or out of range "
+                         f"(status {int(status[bad[0]])}; {len(bad)} problem(s) in all)")
+    return out
