@@ -455,6 +455,79 @@ typedef struct setk_rir_config {
 int setk_rir_image(const setk_rir_config_t* cfg, const double* room, const double* beta, const double* source,
                    const double* receivers, int32_t B, int32_t M, float* rir, uint32_t* status, void* stream);
 
+/* ---- speech + RIR + noise mixture simulation (scripts/sptk/wav_simulate.py; csrc/simu.cu) ---- */
+#define SETK_CONV_MAX_LEN (1 << 24)   /* Sx, Lh and Ny each <= 2^24 samples (17 min at 16 kHz) */
+#define SETK_SIMU_MAX_TERMS 64        /* terms per mixture */
+
+/*
+ * Batched long linear convolution: ss.convolve(spk[None], rir)[..., :S] of add_room_response
+ * (wav_simulate.py:29-54, minus the power) for B problems, each a mono source and an M-channel filter:
+ *   y[b][m][n] = sum_k x[b][n - k] h[b][m][k],  n < n_out_b;  y[b][m][n] = 0 for n_out_b <= n < Ny.
+ *   x  f32 [B][Sx]     source b is x[b][0 .. S_b)
+ *   h  f32 [B][M][Lh]  filter b is h[b][m][0 .. L_b)
+ *   y  f32 [B][M][Ny]  written whole
+ *   s_len_host, h_len_host, n_out_host  i32 [B] on the host, or NULL for Sx, Lh and Ny; n_out_b = S_b
+ *   is the reference's truncation, S_b + L_b - 1 the full convolution (any n_out_b in [1, Ny] is accepted).
+ * Uniformly partitioned overlap-save, 1024-sample blocks, fp32 FFTs in shared memory with exact twiddles;
+ * deterministic (a problem gives the same bits alone and inside a batch).  Scratch (the spectra,
+ * 8 (P + 1) B (ceil(Ny / P) + M ceil(Lh / P)) bytes) is stream-ordered.
+ * SETK_EINVAL: a null pointer; B, M, Sx, Lh or Ny < 1; B or M > 65535; S_b, L_b or n_out_b outside
+ * [1, Sx], [1, Lh], [1, Ny].  SETK_EUNSUPPORTED: Sx, Lh or Ny > SETK_CONV_MAX_LEN.
+ */
+int setk_convolve(const float* x, int32_t Sx, const float* h, int32_t Lh, int32_t B, int32_t M,
+                  const int32_t* s_len_host, const int32_t* h_len_host, const int32_t* n_out_host, float* y,
+                  int32_t Ny, void* stream);
+
+#define SETK_SIMU_SPEAKER 0
+#define SETK_SIMU_POINT_NOISE 1
+#define SETK_SIMU_ISOTROPIC 2
+
+typedef struct setk_simu_term {
+  int64_t src;                     /* offset (floats) of the image's channel 0 in `pool` */
+  int32_t kind;                    /* SETK_SIMU_* */
+  int32_t n_channels;              /* 1 (added to every channel) or the mixture's channel count */
+  int32_t pitch;                   /* floats between the image's channels */
+  int32_t begin, length;           /* the image lands on mixture samples [begin, begin + length) */
+  int32_t repeat;                  /* 1: image sample 0 is added at every one of those samples */
+  int32_t power_begin, power_end;  /* the image's channel-0 samples its power is taken over */
+  int32_t reserved;
+  double level_db;                 /* SDR of a speaker after the first, SNR of a noise */
+} setk_simu_term_t;
+
+typedef struct setk_simu_mix {
+  int32_t first_term, n_terms;     /* its terms: speakers, then point noises, then at most one isotropic */
+  int32_t n_samples, n_channels;   /* mix_nsamps (<= n_pitch) and N (<= M) */
+  double norm_factor;
+} setk_simu_mix_t;
+
+/*
+ * Mixing and normalisation of run_simu (wav_simulate.py:166-312) for B mixtures whose images (the
+ * convolved or raw sources and noises, float32) lie in `pool`:
+ *   - power of every image on its channel 0 over [power_begin, power_end), fp64 (add_room_response :54,
+ *     add_speaker :72, add_point_noise :124, isotropic :295);
+ *   - speaker 0 has coefficient 1, speaker k coeff_snr(P_k, P_0, sdr_k) (:87-92);
+ *   - P_spk = mean over n_samples of the scaled speakers' channel-0 sum (:252-255);
+ *   - every noise coeff_snr(P_noise, P_spk, snr) (:141, :296);
+ *   - mix = (sum of speakers + sum of point noises) + isotropic, per channel and sample, terms added in
+ *     table order in fp64; an image of one channel is added to every channel;
+ *   - factor = norm_factor / (max |mix| + EPSILON) over every channel (:304), and the outputs
+ *       mix    [B][M][n_pitch]  mix times factor (channels >= N and samples >= n_samples are 0),
+ *       spk    [B][K][n_pitch]  channel 0 of each scaled speaker times factor, or NULL,
+ *       noise  [B][n_pitch]     channel 0 of point noises + isotropic times factor, or NULL,
+ *       factor f64 [B]          or NULL,
+ *     float32, or with pcm16 != 0 int16 floor(y * 32768) clipped (write_wav's PCM-16).
+ * The term tables are host arrays, copied on `stream`; nothing synchronises the host.
+ * SETK_EINVAL: a null pointer (pool, tables, mix); B, n_terms, M, K or n_pitch < 1; a mixture with no
+ * speaker, more than K speakers, terms out of order, more than one isotropic term, a term range outside
+ * the table, n_samples outside [1, n_pitch] or n_channels outside [1, M]; a term whose n_channels is
+ * neither 1 nor the mixture's (an isotropic term must have 1), whose samples fall outside
+ * [0, n_samples), whose image or power range falls outside the pool, or an empty power range.
+ * SETK_EUNSUPPORTED: more than SETK_SIMU_MAX_TERMS terms in one mixture.
+ */
+int setk_simulate_mix(const float* pool, int64_t pool_len, const setk_simu_mix_t* mixes_host, int32_t B,
+                      const setk_simu_term_t* terms_host, int32_t n_terms, int32_t M, int32_t K, int32_t n_pitch,
+                      int32_t pcm16, void* mix, void* spk, void* noise, double* factor, void* stream);
+
 /* floor(y * 32768) clipped to int16: the PCM_16 conversion of
  * WaveWriter.write -> write_wav -> soundfile (data_handler.py:600-605,
  * utils.py:45-62; SURVEY.md finding 3).  wave f32 [n], pcm i16 [n]. */

@@ -56,6 +56,21 @@ class RirConfig(Structure):
                 ("hp_filter", c_int32)]
 
 
+CONV_MAX_LEN, SIMU_MAX_TERMS = 1 << 24, 64
+SIMU_SPEAKER, SIMU_POINT_NOISE, SIMU_ISOTROPIC = 0, 1, 2
+
+
+class SimuTerm(Structure):
+    _fields_ = [("src", c_int64), ("kind", c_int32), ("n_channels", c_int32), ("pitch", c_int32),
+                ("begin", c_int32), ("length", c_int32), ("repeat", c_int32), ("power_begin", c_int32),
+                ("power_end", c_int32), ("reserved", c_int32), ("level_db", c_double)]
+
+
+class SimuMix(Structure):
+    _fields_ = [("first_term", c_int32), ("n_terms", c_int32), ("n_samples", c_int32), ("n_channels", c_int32),
+                ("norm_factor", c_double)]
+
+
 class SetkError(RuntimeError):
     """A libsetk_b200 call failed (bad argument or CUDA error)."""
 
@@ -128,6 +143,10 @@ _PROTOTYPES = {
                               c_void_p, c_void_p]),
     "setk_rir_image": (c_int, [POINTER(RirConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32,
                                c_void_p, c_void_p, c_void_p]),
+    "setk_convolve": (c_int, [c_void_p, c_int32, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p,
+                              c_void_p, c_void_p, c_int32, c_void_p]),
+    "setk_simulate_mix": (c_int, [c_void_p, c_int64, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_int32,
+                                  c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)

@@ -727,4 +727,83 @@ int setk_rir_image(const setk_rir_config_t* cfg, const double* room, const doubl
   });
 }
 
+// ---- long convolution and mixture simulation (simu.cu) ----
+int setk_convolve(const float* x, int32_t Sx, const float* h, int32_t Lh, int32_t B, int32_t M,
+                  const int32_t* s_len_host, const int32_t* h_len_host, const int32_t* n_out_host, float* y,
+                  int32_t Ny, void* stream) {
+  if (!x || !h || !y) return fail(SETK_EINVAL, "setk_convolve: null argument");
+  if (B < 1 || M < 1 || Sx < 1 || Lh < 1 || Ny < 1 || B > 65535 || M > 65535)
+    return fail(SETK_EINVAL, "setk_convolve: bad shape B=%d M=%d Sx=%d Lh=%d Ny=%d", B, M, Sx, Lh, Ny);
+  if (Sx > SETK_CONV_MAX_LEN || Lh > SETK_CONV_MAX_LEN || Ny > SETK_CONV_MAX_LEN)
+    return fail(SETK_EUNSUPPORTED, "setk_convolve: Sx=%d Lh=%d Ny=%d: each must be <= %d", Sx, Lh, Ny,
+                SETK_CONV_MAX_LEN);
+  std::vector<int> len((size_t)B * 3);
+  for (int b = 0; b < B; ++b) {
+    const int S = s_len_host ? s_len_host[b] : Sx, L = h_len_host ? h_len_host[b] : Lh;
+    const int n = n_out_host ? n_out_host[b] : Ny;
+    if (S < 1 || S > Sx || L < 1 || L > Lh || n < 1 || n > Ny)
+      return fail(SETK_EINVAL, "setk_convolve: problem %d: S=%d L=%d n_out=%d outside [1, %d], [1, %d], [1, %d]", b,
+                  S, L, n, Sx, Lh, Ny);
+    len[3 * (size_t)b] = S;
+    len[3 * (size_t)b + 1] = L;
+    len[3 * (size_t)b + 2] = n;
+  }
+  const size_t len_bytes = up256(sizeof(int) * len.size());
+  return with_scratch(len_bytes + conv_spectra_bytes(B, M, Lh, Ny), stream, "setk_convolve(workspace)",
+                      "setk_convolve", [&](char* ws) {
+    cudaError_t e = cudaMemcpyAsync(ws, len.data(), sizeof(int) * len.size(), cudaMemcpyHostToDevice,
+                                    static_cast<cudaStream_t>(stream));
+    if (e != cudaSuccess) return e;
+    return run_convolve(x, Sx, h, Lh, B, M, reinterpret_cast<const int*>(ws), y, Ny, ws + len_bytes, stream);
+  });
+}
+
+int setk_simulate_mix(const float* pool, int64_t pool_len, const setk_simu_mix_t* mixes_host, int32_t B,
+                      const setk_simu_term_t* terms_host, int32_t n_terms, int32_t M, int32_t K, int32_t n_pitch,
+                      int32_t pcm16, void* mix, void* spk, void* noise, double* factor, void* stream) {
+  if (!pool || !mixes_host || !terms_host || !mix) return fail(SETK_EINVAL, "setk_simulate_mix: null argument");
+  if (B < 1 || n_terms < 1 || M < 1 || K < 1 || n_pitch < 1 || B > 65535 || pool_len < 1)
+    return fail(SETK_EINVAL, "setk_simulate_mix: bad shape B=%d terms=%d M=%d K=%d n_pitch=%d pool=%lld", B,
+                n_terms, M, K, n_pitch, (long long)pool_len);
+  for (int b = 0; b < B; ++b) {
+    const setk_simu_mix_t& mx = mixes_host[b];
+    if (mx.n_terms > SETK_SIMU_MAX_TERMS)
+      return fail(SETK_EUNSUPPORTED, "setk_simulate_mix: mixture %d has %d terms > %d", b, mx.n_terms,
+                  SETK_SIMU_MAX_TERMS);
+    if (mx.first_term < 0 || mx.n_terms < 1 || mx.first_term > n_terms - mx.n_terms)
+      return fail(SETK_EINVAL, "setk_simulate_mix: mixture %d: terms [%d, +%d) outside the table of %d", b,
+                  mx.first_term, mx.n_terms, n_terms);
+    if (mx.n_samples < 1 || mx.n_samples > n_pitch || mx.n_channels < 1 || mx.n_channels > M)
+      return fail(SETK_EINVAL, "setk_simulate_mix: mixture %d: n_samples=%d n_channels=%d outside [1, %d], [1, %d]",
+                  b, mx.n_samples, mx.n_channels, n_pitch, M);
+    int n_spk = 0, last_kind = SETK_SIMU_SPEAKER;
+    for (int i = 0; i < mx.n_terms; ++i) {
+      const setk_simu_term_t& t = terms_host[mx.first_term + i];
+      if (t.kind < SETK_SIMU_SPEAKER || t.kind > SETK_SIMU_ISOTROPIC || t.kind < last_kind ||
+          (i > 0 && t.kind == SETK_SIMU_ISOTROPIC && last_kind == SETK_SIMU_ISOTROPIC))
+        return fail(SETK_EINVAL, "setk_simulate_mix: mixture %d term %d: kind %d out of order", b, i, t.kind);
+      last_kind = t.kind;
+      n_spk += t.kind == SETK_SIMU_SPEAKER;
+      if (t.n_channels != 1 && (t.n_channels != mx.n_channels || t.kind == SETK_SIMU_ISOTROPIC))
+        return fail(SETK_EINVAL, "setk_simulate_mix: mixture %d term %d: %d channels for a %d-channel mixture", b,
+                    i, t.n_channels, mx.n_channels);
+      if (t.begin < 0 || t.length < 0 || t.begin > mx.n_samples - t.length)
+        return fail(SETK_EINVAL, "setk_simulate_mix: mixture %d term %d: samples [%d, +%d) outside [0, %d)", b, i,
+                    t.begin, t.length, mx.n_samples);
+      const int64_t reach = (int64_t)(t.n_channels - 1) * t.pitch + (t.repeat ? 1 : t.length);
+      if (t.src < 0 || t.pitch < 0 || t.src + reach > pool_len || t.power_begin < 0 ||
+          t.power_end <= t.power_begin || t.src + t.power_end > pool_len)
+        return fail(SETK_EINVAL, "setk_simulate_mix: mixture %d term %d: image or power range outside the pool",
+                    b, i);
+    }
+    if (n_spk < 1 || n_spk > K)
+      return fail(SETK_EINVAL, "setk_simulate_mix: mixture %d has %d speakers, want [1, %d]", b, n_spk, K);
+  }
+  return with_scratch(simu_scratch_bytes(B, n_terms, n_pitch), stream, "setk_simulate_mix(workspace)",
+                      "setk_simulate_mix", [&](char* ws) {
+    return run_simulate_mix(pool, B, n_terms, M, K, n_pitch, pcm16, ws, mixes_host, terms_host, mix, spk, noise,
+                            factor, stream);
+  });
+}
+
 }  // extern "C"

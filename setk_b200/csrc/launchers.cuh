@@ -129,6 +129,16 @@ cudaError_t run_rir_image(const setk_rir_config_t& cfg, const double* room, cons
                           const double* source, const double* receivers, int B, int M, int max_n, float* rir,
                           double* ws, unsigned* status, void* stream);
 
+// ---- simu.cu: long convolution and mixture simulation ----
+int conv_block();
+size_t conv_spectra_bytes(int B, int M, int Lh, int Ny);
+cudaError_t run_convolve(const float* x, int Sx, const float* h, int Lh, int B, int M, const int* len, float* y,
+                         int Ny, char* ws, void* stream);
+size_t simu_scratch_bytes(int B, int n_terms, int n_pitch);
+cudaError_t run_simulate_mix(const float* pool, int B, int n_terms, int M, int K, int n_pitch, int pcm16,
+                             char* ws, const setk_simu_mix_t* mixes_host, const setk_simu_term_t* terms_host,
+                             void* mix, void* spk, void* noise, double* factor, void* stream);
+
 // ---- cm_mask.cu: Kaldi compressed-matrix masks ----
 cudaError_t run_cm_masks(const unsigned char* blobs, long long slot_bytes, int B, int T, int F, float* out,
                          int* status, void* stream);

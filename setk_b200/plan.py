@@ -748,3 +748,86 @@ def rir_image(room, beta, source, receivers, n_samples, sr=16000, c=340, order=-
         raise ValueError(f"rir_image: the response of problem {bad[0]} is not finite or out of range "
                          f"(status {int(status[bad[0]])}; {len(bad)} problem(s) in all)")
     return out
+
+
+# ---------------------------------------------------------------------------
+# Speech + RIR + noise mixtures (wav_simulate.py of the reference; csrc/simu.cu, setk_b200/simu.py)
+# ---------------------------------------------------------------------------
+def _lens(v, B, what):
+    if v is None:
+        return None
+    a = np.ascontiguousarray(np.broadcast_to(np.asarray(v, dtype=np.int32), (B,)))
+    if a.shape != (B,):
+        raise ValueError(f"{what} must be one length or ({B},)")
+    return a
+
+
+def convolve(x, h, n_out=None, s_len=None, h_len=None, out=None):
+    """
+    ss.convolve(x[None], h)[..., :n_out] of add_room_response (wav_simulate.py:29-54, without the
+    power) for B problems: x (B,S) float32 sources, h (B,M,L) float32 filters; one problem may drop
+    the leading B (x (S,), h (M,L) or (L,)).  n_out: None gives S (the reference's truncation), S + L - 1
+    is the full convolution; an int or (B,) per problem.  s_len / h_len: (B,) true lengths of a ragged
+    batch (None: S and L).  Returns y (B,M,Ny) float32, Ny = max n_out, zero past each problem's n_out
+    (or writes `out`, a contiguous (B,M,Ny) float32 tensor).
+    """
+    x, h = torch.as_tensor(x), torch.as_tensor(h)
+    single = x.dim() == 1
+    if single:
+        x = x[None]
+        h = h.reshape(1, 1, -1) if h.dim() == 1 else h[None]
+    if x.dim() != 2 or h.dim() != 3 or h.shape[0] != x.shape[0]:
+        raise ValueError(f"convolve: x {tuple(x.shape)} and h {tuple(h.shape)}: want (B,S) and (B,M,L)")
+    dev = h.device if h.device.type != "cpu" else x.device
+    x = _f32(x, dev).contiguous()
+    h = _f32(h, dev).contiguous()
+    B, Sx = x.shape
+    M, Lh = h.shape[1], h.shape[2]
+    s_l, h_l = _lens(s_len, B, "s_len"), _lens(h_len, B, "h_len")
+    if n_out is None:
+        n_l = s_l if s_l is not None else np.full(B, Sx, np.int32)
+    else:
+        n_l = _lens(n_out, B, "n_out")
+    Ny = int(n_l.max()) if B else 0
+    if out is None:
+        out = torch.empty((B, M, max(Ny, 0)), dtype=torch.float32, device=dev)
+    elif out.shape != (B, M, Ny) or out.dtype != torch.float32 or not out.is_contiguous():
+        raise ValueError(f"convolve: out must be a contiguous float32 ({B}, {M}, {Ny}) tensor")
+
+    def p(a):
+        return None if a is None else a.ctypes.data_as(ctypes.POINTER(ctypes.c_int32))
+
+    with _ctx(dev):
+        _lib.check(_lib.library().setk_convolve(_lib.ptr(x), Sx, _lib.ptr(h), Lh, B, M, p(s_l), p(h_l), p(n_l),
+                                                _lib.ptr(out), Ny, _lib.current_stream(dev)))
+    return out[0] if single else out
+
+
+def simulate_mix(pool, mixes, terms, n_channels, n_speakers, n_samples, pcm16=False, spk=True, noise=True):
+    """
+    Mixing and normalisation of run_simu (wav_simulate.py:166-312) for B mixtures whose images lie in
+    `pool` (a flat float32 tensor).  mixes: B dicts of setk_simu_mix_t (first_term, n_terms, n_samples,
+    n_channels, norm_factor); terms: dicts of setk_simu_term_t (src, kind, n_channels, pitch, begin,
+    length, repeat, power_begin, power_end, level_db).  n_channels, n_speakers, n_samples: the output
+    shape M, K, n_pitch.  Returns (mix (B,M,n_pitch), spk (B,K,n_pitch) or None, noise (B,n_pitch) or
+    None, factor (B,) float64), float32 or, with pcm16, int16 as write_wav stores them.
+    """
+    pool = pool.reshape(-1)
+    if pool.dtype != torch.float32 or not pool.is_contiguous():
+        raise ValueError("simulate_mix: pool must be a contiguous float32 tensor")
+    dev = pool.device
+    B, T = len(mixes), len(terms)
+    mx = (_lib.SimuMix * max(B, 1))(*[_lib.SimuMix(**m) for m in mixes])
+    tm = (_lib.SimuTerm * max(T, 1))(*[_lib.SimuTerm(**t) for t in terms])
+    M, K, N = int(n_channels), int(n_speakers), int(n_samples)
+    dt = torch.int16 if pcm16 else torch.float32
+    mix = torch.empty((B, M, max(N, 0)), dtype=dt, device=dev)
+    s = torch.empty((B, K, max(N, 0)), dtype=dt, device=dev) if spk else None
+    nz = torch.empty((B, max(N, 0)), dtype=dt, device=dev) if noise else None
+    factor = torch.empty((B,), dtype=torch.float64, device=dev)
+    with _ctx(dev):
+        _lib.check(_lib.library().setk_simulate_mix(
+            _lib.ptr(pool), pool.numel(), ctypes.cast(mx, ctypes.c_void_p), B, ctypes.cast(tm, ctypes.c_void_p), T,
+            M, K, N, int(bool(pcm16)), _lib.ptr(mix), _lib.ptr(s), _lib.ptr(nz), _lib.ptr(factor),
+            _lib.current_stream(dev)))
+    return mix, s, nz, factor
