@@ -5,11 +5,11 @@ against the float64 oracle (oracle/auxiva_oracle.py) and the reference fixtures
 (tests/golden/ref_auxiva.npz), and scripts/sptk/apply_auxiva.py against the reference's files.
 """
 import os
-import subprocess
-import sys
 
 import numpy as np
 import torch
+
+from script_runner import run_script
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden", "ref_auxiva.npz")
@@ -99,25 +99,12 @@ def write_cli_inputs(tmp_path, with_silent=True):
     return g
 
 
-def run_cli(argv, library=None):
-    """scripts/sptk/apply_auxiva.py in a fresh interpreter; `library` binds the CPU execution model."""
-    env = dict(os.environ, PYTHONPATH=ROOT)
-    pre = ""
-    if library:
-        env["SETK_B200_TEST_LIBRARY"] = library
-        pre = ("from setk_b200 import _lib; _lib.use_library(os.environ['SETK_B200_TEST_LIBRARY']);"
-               "from setk_b200.libs import utils; utils.set_default_device('cpu');")
-    runner = "import os, sys, runpy; sys.argv = sys.argv[1:];" + pre + "runpy.run_path(sys.argv[0], run_name='__main__')"
-    subprocess.run([sys.executable, "-c", runner, os.path.join(ROOT, "scripts", "sptk", "apply_auxiva.py"), *argv],
-                   check=True, env=env, cwd=ROOT, stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
-
-
 def check_cli(tmp_path, library=None):
     """Every source file within 1 LSB of the reference's; the silent-channel key skipped, the run goes on."""
     import scipy.io.wavfile as wavfile
     g = write_cli_inputs(tmp_path)
     out = tmp_path / "out"
-    run_cli([str(tmp_path / "wav.scp"), str(out)], library)
+    run_script("apply_auxiva.py", [str(tmp_path / "wav.scp"), str(out)], library)
     assert not list(out.glob("silent.*")), "the singular utterance was written"
     stats = {}
     for name in NAMES:

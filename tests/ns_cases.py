@@ -5,11 +5,11 @@ float64 oracle (oracle/ns_oracle.py) and the reference fixtures (tests/golden/re
 scripts/sptk/apply_ns.py against the reference's shipped output.
 """
 import os
-import subprocess
-import sys
 
 import numpy as np
 import torch
+
+from script_runner import run_script
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden", "ref_ns.npz")
@@ -119,26 +119,13 @@ def write_cli_inputs(tmp_path, with_multichannel=True):
     return gold
 
 
-def run_cli(argv, library=None):
-    """scripts/sptk/apply_ns.py in a fresh interpreter; `library` binds the CPU execution model."""
-    env = dict(os.environ, PYTHONPATH=ROOT)
-    pre = ""
-    if library:
-        env["SETK_B200_TEST_LIBRARY"] = library
-        pre = ("from setk_b200 import _lib; _lib.use_library(os.environ['SETK_B200_TEST_LIBRARY']);"
-               "from setk_b200.libs import utils; utils.set_default_device('cpu');")
-    runner = "import os, sys, runpy; sys.argv = sys.argv[1:];" + pre + "runpy.run_path(sys.argv[0], run_name='__main__')"
-    subprocess.run([sys.executable, "-c", runner, os.path.join(ROOT, "scripts", "sptk", "apply_ns.py"), *argv],
-                   check=True, env=env, cwd=ROOT, stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
-
-
 def check_cli(tmp_path, library=None):
     """--output wave: every sample within 1 LSB of the shipped egs_ns.wav, >= 99 % exact; the
     multichannel key skipped.  Returns the exact fraction."""
     import scipy.io.wavfile as wavfile
     gold = write_cli_inputs(tmp_path)
     out = tmp_path / "out"
-    run_cli([str(tmp_path / "wav.scp"), str(out)], library)
+    run_script("apply_ns.py", [str(tmp_path / "wav.scp"), str(out)], library)
     assert not list(out.glob("stereo.*")), "the multichannel key was written"
     sr, got = wavfile.read(str(out / "egs.wav"))
     want = gold["egs/ns_pcm16"]

@@ -13,10 +13,11 @@ Error measure: max |got - want| over the channel's peak |want|, the worst channe
 import json
 import os
 import subprocess
-import sys
 
 import numpy as np
 import torch
+
+from script_runner import run_script
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden")
@@ -100,20 +101,16 @@ def oracle_case(case, receivers=None):
 
 def run_cli(tmp_path, which, extra=(), check_sources=None):
     """
-    runs scripts/sptk/rir_generate_{which}.py (seeded) and checks every file's name, format and
-    shape, and those of the first `check_sources` sources of each room (all when None) against the
-    oracle run on rir.json.  Returns (rir.json, worst |PCM-16 difference| in LSB).
+    runs scripts/sptk/rir_generate_{which}.py for 2 rooms (seeded, in tmp_path, --dump-dir rir) and
+    checks every file's name, format and shape, and those of the first `check_sources` sources of
+    each room (all when None) against the oracle run on rir.json.  Returns (rir.json, worst
+    |PCM-16 difference| in LSB).
     """
     from setk_b200 import _lib
     import scipy.io.wavfile as wavfile
-    script = os.path.join(ROOT, "scripts", "sptk", f"rir_generate_{which}.py")
-    dump = str(tmp_path / f"rir{which}")
-    code = ("import random, runpy, sys; random.seed(7); sys.argv = sys.argv[1:]; "
-            "from setk_b200 import _lib; _lib.use_library(sys.argv.pop(1)); "
-            "runpy.run_path(sys.argv[0], run_name='__main__')")
-    args = [sys.executable, "-c", code, script, _lib.library_path(), "--dump-dir", dump, *extra, "2"]
-    subprocess.run(args, check=True, cwd=ROOT, env=dict(os.environ, PYTHONPATH=ROOT))
-    with open(os.path.join(dump, "rir.json")) as f:
+    run_script(f"rir_generate_{which}.py", ["--dump-dir", "rir", *extra, "2"], library=_lib.library_path(),
+               cwd=tmp_path, seed=7)
+    with open(tmp_path / "rir" / "rir.json") as f:
         cfg = json.load(f)
     assert len(cfg) == 2
     worst = 0
@@ -121,8 +118,8 @@ def run_cli(tmp_path, which, extra=(), check_sources=None):
         assert set(room) == {"beta", "receiver_location", "room_size", "receiver_geometric", "spk"}
         for i, spk in enumerate(room["spk"]):
             assert set(spk) == {"pos", "doa", "dst", "loc"}
-            assert spk["loc"] == f"{dump}/Room{r + 1}-{i + 1}.wav"
-            sr, data = wavfile.read(spk["loc"])
+            assert spk["loc"] == f"rir/Room{r + 1}-{i + 1}.wav"
+            sr, data = wavfile.read(tmp_path / spk["loc"])
             assert sr == 16000 and data.dtype == np.int16 and data.shape[1] == len(room["receiver_location"])
             pcm = data.T
             if check_sources is not None and i >= check_sources:

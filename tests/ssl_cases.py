@@ -4,11 +4,11 @@ model, tests/test_gpu_ssl.py on the device): setk_ssl through setk_b200.plan.ssl
 float64 oracle (oracle/ssl_oracle.py) and the reference fixtures (tests/golden/ref_ssl.npz).
 """
 import os
-import subprocess
-import sys
 
 import numpy as np
 import torch
+
+from script_runner import run_script
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden", "ref_ssl.npz")
@@ -188,24 +188,11 @@ def cli_argv(tmp_path, flags, out):
     return argv + [str(tmp_path / "wav.scp"), str(tmp_path / "sv.npy"), str(out)]
 
 
-def run_cli(argv, library=None):
-    """scripts/sptk/do_ssl.py in a fresh interpreter; `library` binds the CPU execution model."""
-    env = dict(os.environ, PYTHONPATH=ROOT)
-    pre = ""
-    if library:
-        env["SETK_B200_TEST_LIBRARY"] = library
-        pre = ("from setk_b200 import _lib; _lib.use_library(os.environ['SETK_B200_TEST_LIBRARY']);"
-               "from setk_b200.libs import utils; utils.set_default_device('cpu');")
-    runner = "import os, sys, runpy; sys.argv = sys.argv[1:];" + pre + "runpy.run_path(sys.argv[0], run_name='__main__')"
-    subprocess.run([sys.executable, "-c", runner, os.path.join(ROOT, "scripts", "sptk", "do_ssl.py"), *argv],
-                   check=True, env=env, cwd=ROOT, stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
-
-
 def check_cli(tmp_path, library=None):
     g = write_cli_inputs(tmp_path)
     for run in CLI_RUNS:
         out = tmp_path / f"{run}.txt"
-        run_cli(cli_argv(tmp_path, str(g[f"cli/{run}/flags"]), out), library)
+        run_script("do_ssl.py", cli_argv(tmp_path, str(g[f"cli/{run}/flags"]), out), library)
         assert out.read_text() == str(g[f"cli/{run}/doa_scp"]), f"do_ssl.py {run}: output differs"
 
 
@@ -214,8 +201,9 @@ def check_cli_online_mask(tmp_path, library=None):
     chunk's frames of the STFT and of the mask."""
     g = write_cli_inputs(tmp_path)
     out = tmp_path / "online_mask.txt"
-    run_cli(["--chunk-len", "6", "--look-back", "9", "--mask-scp", str(tmp_path / "mask2.scp"),
-             "--doa-range", "0,180", str(tmp_path / "wav.scp"), str(tmp_path / "sv.npy"), str(out)], library)
+    run_script("do_ssl.py", ["--chunk-len", "6", "--look-back", "9", "--mask-scp", str(tmp_path / "mask2.scp"),
+                             "--doa-range", "0,180", str(tmp_path / "wav.scp"), str(tmp_path / "sv.npy"), str(out)],
+               library)
     lines = dict(line.split("\t") for line in out.read_text().splitlines())
     labels = so.doa_labels(0, 180, g["cli/sv"].shape[0], "degree")
     for key in ("utt0", "utt1"):

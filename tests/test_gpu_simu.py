@@ -5,8 +5,6 @@ mixtures of mixed shapes (bit-identical run to run and to each mixture alone) an
 --batch on the doc commands.
 """
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -14,6 +12,7 @@ import scipy.io.wavfile as wavfile
 import torch
 
 import simu_cases as sc
+from script_runner import run_script
 
 pytestmark = pytest.mark.gpu
 
@@ -109,12 +108,7 @@ def test_command_line_batch_vs_reference(cuda, golden_dir, tmp_path):
         lines.append(" ".join(argv))
     listing = tmp_path / "list.txt"
     listing.write_text("\n".join(lines) + "\n")
-    code = ("import runpy, sys; sys.argv = sys.argv[1:]; from setk_b200 import _lib; "
-            "_lib.use_library(sys.argv.pop(1)); runpy.run_path(sys.argv[0], run_name='__main__')")
-    script = os.path.join(sc.ROOT, "scripts", "sptk", "wav_simulate.py")
-    out = subprocess.run([sys.executable, "-c", code, script, _lib.library_path(), "--batch", str(listing)],
-                         check=True, cwd=str(tmp_path), env=dict(os.environ, PYTHONPATH=sc.ROOT),
-                         capture_output=True, text=True).stdout
+    out = run_script("wav_simulate.py", ["--batch", str(listing)], _lib.library_path(), cwd=tmp_path).stdout
     assert out.count("RTF = ") == len(names)
     for name in names:
         flags = sc.case_flags(STORE, name)

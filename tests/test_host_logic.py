@@ -4,8 +4,6 @@ the batched engine and the CLI) running on the CPU execution model of the
 kernels, against the oracle.
 """
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -13,8 +11,7 @@ import torch
 
 from oracle import beamformer_oracle as bo
 from oracle import stft_oracle as so
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from script_runner import run_script
 
 
 @pytest.fixture()
@@ -141,12 +138,6 @@ def test_cli_end_to_end(tmp_path, emu_library_path):
     np.save(tmp_path / "utt1.npy", m)
     (tmp_path / "wav.scp").write_text(f"utt1 {tmp_path / 'utt1.wav'}\n")
     (tmp_path / "mask.scp").write_text(f"utt1 {tmp_path / 'utt1.npy'}\n")
-    env = dict(os.environ, SETK_B200_TEST_LIBRARY=emu_library_path, PYTHONPATH=ROOT)
-    runner = (
-        "import os, sys, runpy; sys.argv = sys.argv[1:];"
-        "from setk_b200 import _lib; _lib.use_library(os.environ['SETK_B200_TEST_LIBRARY']);"
-        "from setk_b200.libs import utils; utils.set_default_device('cpu');"
-        "runpy.run_path(sys.argv[0], run_name='__main__')")
     import scipy.io.wavfile as wavfile
     # PMWF is phase invariant, so the waveform itself is comparable with the oracle;
     # MVDR's per-bin sign is LAPACK-defined in the reference (checked elsewhere after alignment)
@@ -155,13 +146,11 @@ def test_cli_end_to_end(tmp_path, emu_library_path):
              ("mvdr", ["--post-masking", "true"], None))
     for bf, extra, okw in cases:
         dst = tmp_path / bf
-        cmd = [sys.executable, "-c", runner,
-               os.path.join(ROOT, "scripts", "sptk", "apply_adaptive_beamformer.py"),
-               "--frame-len", "512", "--frame-hop", "256", "--mask-format", "numpy",
-               "--batch-size", "0",       # the batched feeder needs CUDA streams: tests/test_gpu_cli.py
-               "--beamformer", bf, *extra, str(tmp_path / "wav.scp"), str(tmp_path / "mask.scp"),
-               str(dst)]
-        subprocess.run(cmd, check=True, env=env, capture_output=True)
+        run_script("apply_adaptive_beamformer.py",
+                   ["--frame-len", "512", "--frame-hop", "256", "--mask-format", "numpy",
+                    "--batch-size", "0",       # the batched feeder needs CUDA streams: tests/test_gpu_cli.py
+                    "--beamformer", bf, *extra, str(tmp_path / "wav.scp"), str(tmp_path / "mask.scp"),
+                    str(dst)], emu_library_path)
         sr, out = wavfile.read(str(dst / "utt1.wav"))
         assert sr == 16000 and out.dtype == np.int16
         assert out.shape == (256 * (so.num_frames(4000, 512, 256, True) - 1),)
@@ -222,16 +211,9 @@ def test_cgmm_trainer_mirror_and_cli(tmp_path, emu, emu_library_path):
     # (b) the CLI, documented flags, from a wav file
     _write_wav(str(tmp_path / "utt1.wav"), x)
     (tmp_path / "wav.scp").write_text(f"utt1 {tmp_path / 'utt1.wav'}\n")
-    env = dict(os.environ, SETK_B200_TEST_LIBRARY=emu_library_path, PYTHONPATH=ROOT)
-    runner = (
-        "import os, sys, runpy; sys.argv = sys.argv[1:];"
-        "from setk_b200 import _lib; _lib.use_library(os.environ['SETK_B200_TEST_LIBRARY']);"
-        "from setk_b200.libs import utils; utils.set_default_device('cpu');"
-        "runpy.run_path(sys.argv[0], run_name='__main__')")
-    cmd = [sys.executable, "-c", runner, os.path.join(ROOT, "scripts", "sptk", "estimate_cgmm_masks.py"),
-           "--frame-len", "512", "--frame-hop", "256", "--num-iters", "3", "--center", "true",
-           str(tmp_path / "wav.scp"), str(tmp_path / "masks")]
-    subprocess.run(cmd, check=True, env=env, capture_output=True)
+    run_script("estimate_cgmm_masks.py",
+               ["--frame-len", "512", "--frame-hop", "256", "--num-iters", "3", "--center", "true",
+                str(tmp_path / "wav.scp"), str(tmp_path / "masks")], emu_library_path)
     mask = np.load(tmp_path / "masks" / "utt1.npy")
     T = so.num_frames(3000, 512, 256, True)
     assert mask.shape == (T, 257) and mask.dtype == np.float32
@@ -265,16 +247,9 @@ def test_wpe_mirror_and_cli(tmp_path, emu, emu_library_path):
     # the CLI: all channels of the dereverberated signal as one PCM-16 file
     _write_wav(str(tmp_path / "utt1.wav"), x)
     (tmp_path / "wav.scp").write_text(f"utt1 {tmp_path / 'utt1.wav'}\n")
-    env = dict(os.environ, SETK_B200_TEST_LIBRARY=emu_library_path, PYTHONPATH=ROOT)
-    runner = (
-        "import os, sys, runpy; sys.argv = sys.argv[1:];"
-        "from setk_b200 import _lib; _lib.use_library(os.environ['SETK_B200_TEST_LIBRARY']);"
-        "from setk_b200.libs import utils; utils.set_default_device('cpu');"
-        "runpy.run_path(sys.argv[0], run_name='__main__')")
-    cmd = [sys.executable, "-c", runner, os.path.join(ROOT, "scripts", "sptk", "apply_wpe.py"),
-           "--frame-len", "256", "--frame-hop", "64", "--center", "true", "--taps", "4", "--delay", "2",
-           "--num-iters", "2", str(tmp_path / "wav.scp"), str(tmp_path / "out")]
-    subprocess.run(cmd, check=True, env=env, capture_output=True)
+    run_script("apply_wpe.py",
+               ["--frame-len", "256", "--frame-hop", "64", "--center", "true", "--taps", "4", "--delay", "2",
+                "--num-iters", "2", str(tmp_path / "wav.scp"), str(tmp_path / "out")], emu_library_path)
     import scipy.io.wavfile as wavfile
     sr, y = wavfile.read(str(tmp_path / "out" / "utt1.wav"))
     assert sr == 16000 and y.dtype == np.int16 and y.shape[1] == 2
@@ -348,15 +323,7 @@ def test_archive_writer_and_spatial_cli(tmp_path, emu, emu_library_path):
     # ---- the CLI, the reference's flags, all three feature types ----
     _write_wav(str(tmp_path / "utt1.wav"), x)
     (tmp_path / "wav.scp").write_text(f"utt1 {tmp_path / 'utt1.wav'}\n")
-    env = dict(os.environ, SETK_B200_TEST_LIBRARY=emu_library_path, PYTHONPATH=ROOT)
-    runner = (
-        "import os, sys, runpy; sys.argv = sys.argv[1:];"
-        "from setk_b200 import _lib; _lib.use_library(os.environ['SETK_B200_TEST_LIBRARY']);"
-        "from setk_b200.libs import utils; utils.set_default_device('cpu');"
-        "runpy.run_path(sys.argv[0], run_name='__main__')")
-    script = os.path.join(ROOT, "scripts", "sptk", "compute_ipd_and_linear_srp.py")
-    base = [sys.executable, "-c", runner, script, "--frame-len", "128", "--frame-hop", "64",
-            "--center", "true"]
+    stft = ["--frame-len", "128", "--frame-hop", "64", "--center", "true"]
     cases = {
         "srp": (["--type", "srp", "--srp.topo", "0,0.1,0.25", "--srp.num_doa", "21"], ref_srp),
         "ipd": (["--type", "ipd", "--ipd.pair", "0,1;0,2", "--ipd.cos", "true"],
@@ -365,20 +332,18 @@ def test_archive_writer_and_spatial_cli(tmp_path, emu, emu_library_path):
     }
     for name, (flags, ref) in cases.items():
         ark, scp = tmp_path / f"{name}.ark", tmp_path / f"{name}.scp"
-        subprocess.run(base + flags + ["--scp", str(scp), str(tmp_path / "wav.scp"), str(ark)], check=True,
-                       env=env, capture_output=True)
+        run_script("compute_ipd_and_linear_srp.py", stft + flags + ["--scp", str(scp), str(tmp_path / "wav.scp"),
+                                                                    str(ark)], emu_library_path)
         feats = ScriptReader(str(scp))["utt1"]
         assert feats.dtype == np.float32 and feats.shape == ref.shape, (name, feats.shape, ref.shape)
         assert np.max(np.abs(feats - ref)) <= 1e-5 * max(1.0, np.max(np.abs(ref))), name
     # ---- directional features from given steer vectors / from a TF-mask ----
     A = np.exp(1j * rng.uniform(0, 6.28, size=(3, 3, F)))                          # A x M x F
     np.save(str(tmp_path / "sv.npy"), A)
-    script = os.path.join(ROOT, "scripts", "sptk", "compute_df_on_geometry.py")
-    base = [sys.executable, "-c", runner, script, "--frame-len", "128", "--frame-hop", "64", "--center", "true"]
     ark, scp = tmp_path / "dfg.ark", tmp_path / "dfg.scp"
-    subprocess.run(base + ["--doa-idx", "0,2", "--df-pair", "0,1;0,2", "--scp", str(scp),
-                           str(tmp_path / "wav.scp"), str(tmp_path / "sv.npy"), str(ark)],
-                   check=True, env=env, capture_output=True)
+    run_script("compute_df_on_geometry.py", stft + ["--doa-idx", "0,2", "--df-pair", "0,1;0,2", "--scp", str(scp),
+                                                    str(tmp_path / "wav.scp"), str(tmp_path / "sv.npy"), str(ark)],
+               emu_library_path)
     dfs = np.stack([sp.directional_feats(obs, A[i], df_pair=[(0, 1), (0, 2)]) for i in (0, 2)])
     ref = dfs.transpose(1, 0, 2).reshape(dfs.shape[1], -1)
     feats = ScriptReader(str(scp))["utt1"]
@@ -386,24 +351,20 @@ def test_archive_writer_and_spatial_cli(tmp_path, emu, emu_library_path):
     mask = rng.uniform(0.05, 1.0, size=(S.shape[1], F)).astype(np.float32)         # T x F
     np.save(str(tmp_path / "mask.npy"), mask)
     (tmp_path / "mask.scp").write_text(f"utt1 {tmp_path / 'mask.npy'}\n")
-    script = os.path.join(ROOT, "scripts", "sptk", "compute_df_on_mask.py")
-    base = [sys.executable, "-c", runner, script, "--frame-len", "128", "--frame-hop", "64", "--center", "true"]
     ark, scp = tmp_path / "dfm.ark", tmp_path / "dfm.scp"
-    subprocess.run(base + ["--mask-format", "numpy", "--df-pair", "0,2", "--scp", str(scp),
-                           str(tmp_path / "wav.scp"), str(tmp_path / "mask.scp"), str(ark)],
-                   check=True, env=env, capture_output=True)
+    run_script("compute_df_on_mask.py", stft + ["--mask-format", "numpy", "--df-pair", "0,2", "--scp", str(scp),
+                                                str(tmp_path / "wav.scp"), str(tmp_path / "mask.scp"), str(ark)],
+               emu_library_path)
     Rs = bo.compute_covar(obs.astype(np.complex128), mask.astype(np.float64))
     sv = bo.solve_pevd(Rs)                                                          # F x N (phase: arbitrary)
     ref = sp.directional_feats(obs, sv.T, df_pair=[(0, 2)])      # phase differences: sign/phase invariant
     feats = ScriptReader(str(scp))["utt1"]
     assert feats.shape == ref.shape and np.max(np.abs(feats - ref)) <= 2e-4
     # ---- SRP for a circular array: mean of the diagonal pairs' GCC-PHAT ----
-    script = os.path.join(ROOT, "scripts", "sptk", "compute_circular_srp.py")
-    base = [sys.executable, "-c", runner, script, "--frame-len", "128", "--frame-hop", "64", "--center", "true"]
     ark, scp = tmp_path / "csrp.ark", tmp_path / "csrp.scp"
-    subprocess.run(base + ["--n", "3", "--d", "0.08", "--diag-pair", "0,2;1,2", "--num-doas", "17",
-                           "--scp", str(scp), str(tmp_path / "wav.scp"), str(ark)],
-                   check=True, env=env, capture_output=True)
+    run_script("compute_circular_srp.py", stft + ["--n", "3", "--d", "0.08", "--diag-pair", "0,2;1,2",
+                                                  "--num-doas", "17", "--scp", str(scp), str(tmp_path / "wav.scp"),
+                                                  str(ark)], emu_library_path)
     ref = np.average(np.stack([sp.gcc_phat_diag(S[i], S[j], min(i, j) * np.pi * 2 / 3, 0.08, num_bins=F,
                                                 sr=16000, num_doas=17) for i, j in ((0, 2), (1, 2))]), axis=0)
     feats = ScriptReader(str(scp))["utt1"]
@@ -431,19 +392,13 @@ def test_geometry_based_beamformers(libs, tmp_path, emu_library_path):
     _write_wav(str(tmp_path / "utt1.wav"), x)
     (tmp_path / "wav.scp").write_text(f"utt1 {tmp_path / 'utt1.wav'}\n")
     (tmp_path / "beam.scp").write_text("utt1 1\n")
-    env = dict(os.environ, SETK_B200_TEST_LIBRARY=emu_library_path, PYTHONPATH=ROOT)
-    runner = (
-        "import os, sys, runpy; sys.argv = sys.argv[1:];"
-        "from setk_b200 import _lib; _lib.use_library(os.environ['SETK_B200_TEST_LIBRARY']);"
-        "from setk_b200.libs import utils; utils.set_default_device('cpu');"
-        "runpy.run_path(sys.argv[0], run_name='__main__')")
-    script = os.path.join(ROOT, "scripts", "sptk", "apply_fixed_beamformer.py")
-    base = [sys.executable, "-c", runner, script, "--frame-len", "256", "--frame-hop", "128", "--center", "true"]
+    stft = ["--frame-len", "256", "--frame-hop", "128", "--center", "true"]
     import scipy.io.wavfile as wavfile
     for tag, wfile, extra, w in (("single", "w_single.npy", [], w0),
                                  ("multi", "w_multi.npy", ["--beam", str(tmp_path / "beam.scp")], w1)):
-        subprocess.run(base + extra + [str(tmp_path / "wav.scp"), str(tmp_path / wfile), str(tmp_path / tag)],
-                       check=True, env=env, capture_output=True)
+        run_script("apply_fixed_beamformer.py",
+                   stft + extra + [str(tmp_path / "wav.scp"), str(tmp_path / wfile), str(tmp_path / tag)],
+                   emu_library_path)
         sr, y = wavfile.read(str(tmp_path / tag / "utt1.wav"))
         enh = np.einsum("fn,nft->ft", w.conj(), obs.astype(np.complex128))
         yo = so.inverse_stft(enh, frame_len=256, frame_hop=128, center=True, window="hann", transpose=False,
@@ -452,9 +407,7 @@ def test_geometry_based_beamformers(libs, tmp_path, emu_library_path):
         assert sr == 16000 and y.dtype == np.int16 and d.max() <= 1, (tag, int(d.max()))
     # scripts/sptk/apply_classic_beamformer.py: SD for a linear array (one DoA per utterance) and
     # DS in chunks (online: one DoA per --chunk-len frames), --normalize true
-    script = os.path.join(ROOT, "scripts", "sptk", "apply_classic_beamformer.py")
-    base = [sys.executable, "-c", runner, script, "--frame-len", "256", "--frame-hop", "128", "--center", "true",
-            "--linear-topo", "0,0.06,0.12", "--normalize", "true"]
+    classic = stft + ["--linear-topo", "0,0.06,0.12", "--normalize", "true"]
     T = obs.shape[-1]
     (tmp_path / "utt2doa").write_text("utt1 70\n")
     half = (T + 1) // 2
@@ -470,8 +423,8 @@ def test_geometry_based_beamformers(libs, tmp_path, emu_library_path):
             o = obs.astype(np.complex128)
             enh = np.hstack([np.einsum("fn,nft->ft", ds.weight(30.0, F, c=343).conj(), o[:, :, :half]),
                              np.einsum("fn,nft->ft", ds.weight(150.0, F, c=343).conj(), o[:, :, half:])])
-        subprocess.run(base + extra + [str(tmp_path / "wav.scp"), str(tmp_path / tag)], check=True, env=env,
-                       capture_output=True)
+        run_script("apply_classic_beamformer.py", classic + extra + [str(tmp_path / "wav.scp"), str(tmp_path / tag)],
+                   emu_library_path)
         sr, y = wavfile.read(str(tmp_path / tag / "utt1.wav"))
         yo = so.inverse_stft(enh, frame_len=256, frame_hop=128, center=True, window="hann", transpose=False,
                              norm=float(np.max(np.abs(x))))
@@ -499,17 +452,10 @@ def test_apply_wpd_cli(tmp_path, emu, emu_library_path):
     x = so.float_from_pcm16(so.pcm16_from_float(x))
     _write_wav(str(tmp_path / "utt1.wav"), x)
     (tmp_path / "wav.scp").write_text(f"utt1 {tmp_path / 'utt1.wav'}\n")
-    env = dict(os.environ, SETK_B200_TEST_LIBRARY=emu_library_path, PYTHONPATH=ROOT)
-    runner = (
-        "import os, sys, runpy; sys.argv = sys.argv[1:];"
-        "from setk_b200 import _lib; _lib.use_library(os.environ['SETK_B200_TEST_LIBRARY']);"
-        "from setk_b200.libs import utils; utils.set_default_device('cpu');"
-        "runpy.run_path(sys.argv[0], run_name='__main__')")
-    cmd = [sys.executable, "-c", runner, os.path.join(ROOT, "scripts", "sptk", "apply_wpd.py"),
-           "--frame-len", "256", "--frame-hop", "64", "--center", "true", "--taps", "3", "--delay", "2",
-           "--wpd-iters", "2", "--cgmm-iters", "3", "--dump-mask", "true",
-           str(tmp_path / "wav.scp"), str(tmp_path / "out")]
-    subprocess.run(cmd, check=True, env=env, capture_output=True)
+    run_script("apply_wpd.py",
+               ["--frame-len", "256", "--frame-hop", "64", "--center", "true", "--taps", "3", "--delay", "2",
+                "--wpd-iters", "2", "--cgmm-iters", "3", "--dump-mask", "true",
+                str(tmp_path / "wav.scp"), str(tmp_path / "out")], emu_library_path)
     kw = dict(frame_len=256, frame_hop=64, center=True, window="hann", round_power_of_two=True, transpose=True)
     obs = so.multichannel_stft(x, out_dtype=np.complex64, **kw)                    # N x T x F
     m_ref, e_ref = wo.facted_wpd(obs, cgmm_iters=3, wpd_iters=2, taps=3, delay=2, context=1)

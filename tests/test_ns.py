@@ -12,6 +12,7 @@ import torch
 
 import ns_cases as nc
 from oracle import ns_oracle as no
+from script_runner import run_script
 
 G = nc.load_fixture()
 
@@ -156,8 +157,8 @@ def test_emu_apply_ns_gain_and_conf(tmp_path, emu_library_path):
     conf = dict(nc.CASE_B_CONF)
     (tmp_path / "ns.yaml").write_text(yaml.safe_dump(conf))
     out = tmp_path / "gain"
-    nc.run_cli([str(tmp_path / "wav.scp"), str(out), "--output", "gain", "--conf", str(tmp_path / "ns.yaml")],
-               emu_library_path)
+    run_script("apply_ns.py", [str(tmp_path / "wav.scp"), str(out), "--output", "gain", "--conf",
+                               str(tmp_path / "ns.yaml")], emu_library_path)
     assert not list(out.glob("stereo.*"))
     g = np.load(out / "egs.npy")
     from oracle import stft_oracle
@@ -172,7 +173,7 @@ def test_emu_apply_ns_gain_and_conf(tmp_path, emu_library_path):
 
 
 def test_apply_ns_rejects_other_sample_rates(tmp_path, emu_library_path):
-    import subprocess
     nc.write_cli_inputs(tmp_path, with_multichannel=False)
-    with pytest.raises(subprocess.CalledProcessError):
-        nc.run_cli([str(tmp_path / "wav.scp"), str(tmp_path / "out"), "--sr", "8000"], emu_library_path)
+    with pytest.raises(AssertionError, match="ValueError: Now only support audio in 16kHz"):
+        run_script("apply_ns.py", [str(tmp_path / "wav.scp"), str(tmp_path / "out"), "--sr", "8000"],
+                   emu_library_path)

@@ -10,8 +10,6 @@ many partitions.
 import argparse
 import ctypes
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -20,6 +18,7 @@ import torch
 
 import rir_cases
 import simu_cases as sc
+from script_runner import run_script
 
 STORE = sc.load_fixture()
 PIN = sc.load_pinning()["oracle_vs_reference"]
@@ -308,11 +307,7 @@ def test_simulate_mix_unsupported_and_smallest(emu):
 
 def _run_cli(argv, cwd):
     from setk_b200 import _lib
-    code = ("import runpy, sys; sys.argv = sys.argv[1:]; from setk_b200 import _lib; "
-            "_lib.use_library(sys.argv.pop(1)); runpy.run_path(sys.argv[0], run_name='__main__')")
-    script = os.path.join(sc.ROOT, "scripts", "sptk", "wav_simulate.py")
-    return subprocess.run([sys.executable, "-c", code, script, _lib.library_path(), *argv], check=True, cwd=cwd,
-                          env=dict(os.environ, PYTHONPATH=sc.ROOT), capture_output=True, text=True).stdout
+    return run_script("wav_simulate.py", argv, _lib.library_path(), cwd=cwd).stdout
 
 
 def _outputs(folder, name, flags):
