@@ -7,7 +7,8 @@
  *
  * and the front ends around it: CGMM masks, WPE / WPD, spatial features, sound
  * source localisation, AuxIVA blind source separation, iMCRA / OM-LSA
- * noise suppression and image-method room impulse responses.
+ * noise suppression, image-method room impulse responses, mixture simulation
+ * and the separation metrics (BSS-Eval SDR / SIR / SAR, SI-SNR).
  *
  * Every entry point below replaces one reference interface; the citation is
  * the reference file:line (paths relative to the reference tree).  The Python
@@ -68,6 +69,7 @@ extern "C" {
 #define SETK_ST_REGULARIZED 32u /* WARNING only: Rn was numerically not PD in a GEV reduction and its
                                    diagonal was loaded (the reference falls back to a non-Hermitian eig
                                    there, beamformer.py:55-58) */
+#define SETK_ST_SILENT 64u      /* a reference or estimate is all zeros (mir_eval's ValueError, setk_bss_eval) */
 
 /* ---- beamformer kinds: apply_adaptive_beamformer.py:22,92-110 ---- */
 #define SETK_BF_MVDR 0          /* beamformer.py:527-539 */
@@ -527,6 +529,57 @@ typedef struct setk_simu_mix {
 int setk_simulate_mix(const float* pool, int64_t pool_len, const setk_simu_mix_t* mixes_host, int32_t B,
                       const setk_simu_term_t* terms_host, int32_t n_terms, int32_t M, int32_t K, int32_t n_pitch,
                       int32_t pcm16, void* mix, void* spk, void* noise, double* factor, void* stream);
+
+/* ---- separation metrics (scripts/sptk/compute_sdr.py, compute_si_snr.py, libs/metric.py; csrc/sep_eval.cu) ---- */
+#define SETK_SEP_MAX_SOURCES 8          /* N in [1, 8] */
+#define SETK_SEP_MAX_FLEN 512           /* L in [1, 512] (mir_eval's bss_eval_sources uses 512) */
+#define SETK_SEP_MAX_COLS 4096          /* N * L <= 4096: the least-squares system is N L square */
+#define SETK_SEP_MAX_SAMPLES (1 << 24)  /* S <= 2^24 samples (17 min at 16 kHz) */
+
+/*
+ * BSS-Eval v3 sources criteria: what mir_eval.separation.bss_eval_sources(ref, sep) computes for
+ * compute_sdr.py:63-80 (its _bss_decomp_mtifilt, _project and _bss_source_crit), for every (estimate j,
+ * reference i) pair of B utterances, with the filter length L:
+ *   est, ref   f32 [B][N][S]     utterance b is [.][.][0 .. n_b)
+ *   n_samples_host  i32 [B] on the host, or NULL for S; each n_b in [1, S]
+ *   crit       f64 [B][3][N][N]  SDR, SIR, SAR of estimate j against reference i at [b][k][j][i]
+ *   dropped    i32 [B] or NULL   columns of the N L square least-squares system found dependent
+ *   status     u32 [B]           written: SETK_ST_SILENT when a reference or estimate is all zeros (the
+ *                                criteria are then meaningless), SETK_ST_NONFINITE for a NaN criterion
+ * With A_i the delayed copies s_i[n - a], a < L, of reference i over n < n_b + L - 1, P_all(j) is
+ * estimate j's least-squares projection onto every A_i and P_spat(j, i) onto A_i alone:
+ *   SDR = 10 log10(|P_spat|^2 / |e_j - P_spat|^2), SIR = 10 log10(|P_spat|^2 / |P_all - P_spat|^2),
+ *   SAR = 10 log10(|P_all|^2 / |e_j - P_all|^2), +inf when the denominator is 0.
+ * Differences from mir_eval: the correlations are direct fp64 sums, not float64 FFTs; the normal
+ * equations are solved by Cholesky, and a column whose pivot is <= 1e-10 of its original diagonal is
+ * dropped, so dependent references (where numpy.linalg.solve is ill-posed) still give the least-squares
+ * projection; the residual energies come from the signals.  The permutation search is the caller's
+ * (setk_b200.libs.metric).  Deterministic: an utterance gives the same bits alone as inside a batch.
+ * Scratch, setk_bss_eval_scratch_bytes(B, N, S, L): about 8 B (N L)^2 bytes for the system plus
+ * 8 B (N L (4 N + 2) + 24 N (N + 1) (S + L) / 256) bytes; it is stream-ordered.
+ * SETK_EINVAL: a null pointer (est, ref, crit, status); B, N, S or L < 1; B > 65535; an n_b outside
+ * [1, S].  SETK_EUNSUPPORTED: N > SETK_SEP_MAX_SOURCES, L > SETK_SEP_MAX_FLEN, N L > SETK_SEP_MAX_COLS,
+ * S > SETK_SEP_MAX_SAMPLES.
+ */
+int setk_bss_eval(const float* est, const float* ref, const int32_t* n_samples_host, int32_t B, int32_t N, int32_t S,
+                  int32_t L, double* crit, int32_t* dropped, uint32_t* status, void* stream);
+/* Bytes of device scratch setk_bss_eval allocates for these sizes (callers that split a batch to bound
+ * it ask here); -1 when setk_bss_eval would reject the sizes. */
+int64_t setk_bss_eval_scratch_bytes(int32_t B, int32_t N, int32_t S, int32_t L);
+
+/*
+ * SI-SNR of every (estimate j, reference i) pair: si_snr(x, s, eps, remove_dc) of libs/metric.py:13-34,
+ * as compute_si_snr.py:82-106 and permute_si_snr (:37-60) call it:
+ *   20 log10(|t| / (|x' - t| + eps) + eps),  t = <x', s'> s' / (|s'|^2 + eps),
+ * x', s' the estimate and reference less their means when remove_dc != 0.
+ *   est, ref   f32 [B][N][S]; n_samples_host as for setk_bss_eval
+ *   out        f64 [B][N][N]     at [b][j][i]
+ * fp64 throughout (the reference computes in float32); |x' - t| is taken from the residual's samples.
+ * SETK_EINVAL: a null pointer; B, N or S < 1; B > 65535; eps < 0 or not finite; an n_b outside [1, S].
+ * SETK_EUNSUPPORTED: N > SETK_SEP_MAX_SOURCES, S > SETK_SEP_MAX_SAMPLES.
+ */
+int setk_si_snr(const float* est, const float* ref, const int32_t* n_samples_host, int32_t B, int32_t N, int32_t S,
+                int32_t remove_dc, double eps, double* out, void* stream);
 
 /* floor(y * 32768) clipped to int16: the PCM_16 conversion of
  * WaveWriter.write -> write_wav -> soundfile (data_handler.py:600-605,

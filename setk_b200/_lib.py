@@ -23,6 +23,8 @@ SETK_MAX_CHANNELS = 16
 SETK_EINVAL, SETK_ENOMEM, SETK_ESHAPE, SETK_EUNSUPPORTED = -1, -2, -3, -4
 ST_SINGULAR, ST_NOT_PD, ST_NO_CONVERGE, ST_NONFINITE, ST_BAD_REF = 1, 2, 4, 8, 16
 ST_REGULARIZED = 32          # warning only
+ST_SILENT = 64               # setk_bss_eval: a reference or estimate is all zeros
+SEP_MAX_SOURCES, SEP_MAX_FLEN, SEP_MAX_COLS, SEP_MAX_SAMPLES = 8, 512, 4096, 1 << 24
 ST_ERROR_MASK = 31
 BF_MVDR, BF_MPDR, BF_MPDR_WHITEN, BF_GEVD, BF_PMWF, BF_PEVD = 0, 1, 2, 3, 4, 5
 RANK1_NONE, RANK1_EIG, RANK1_GEV = 0, 1, 2
@@ -147,6 +149,11 @@ _PROTOTYPES = {
                               c_void_p, c_void_p, c_int32, c_void_p]),
     "setk_simulate_mix": (c_int, [c_void_p, c_int64, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_int32,
                                   c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "setk_bss_eval": (c_int, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p,
+                              c_void_p, c_void_p]),
+    "setk_bss_eval_scratch_bytes": (c_int64, [c_int32, c_int32, c_int32, c_int32]),
+    "setk_si_snr": (c_int, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_double, c_void_p,
+                            c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_PROTOTYPES)

@@ -806,4 +806,68 @@ int setk_simulate_mix(const float* pool, int64_t pool_len, const setk_simu_mix_t
   });
 }
 
+// ---- separation metrics (sep_eval.cu) ----
+// n_b of every utterance into `len` (checked against [1, S])
+static int sep_lengths(const char* who, const int32_t* n_samples_host, int B, int S, std::vector<int>& len) {
+  len.resize((size_t)B);
+  for (int b = 0; b < B; ++b) {
+    len[b] = n_samples_host ? n_samples_host[b] : S;
+    if (len[b] < 1 || len[b] > S)
+      return fail(SETK_EINVAL, "%s: utterance %d has %d samples, want [1, %d]", who, b, len[b], S);
+  }
+  return SETK_OK;
+}
+
+static size_t bss_eval_scratch(int B, int N, int S, int L) {
+  return up256(sizeof(int) * B) + sep_eval_scratch_bytes(B, N, S, L);
+}
+
+int64_t setk_bss_eval_scratch_bytes(int32_t B, int32_t N, int32_t S, int32_t L) {
+  if (B < 1 || N < 1 || S < 1 || L < 1 || B > 65535 || N > SETK_SEP_MAX_SOURCES || L > SETK_SEP_MAX_FLEN ||
+      N * L > SETK_SEP_MAX_COLS || S > SETK_SEP_MAX_SAMPLES)
+    return -1;
+  return (int64_t)bss_eval_scratch(B, N, S, L);
+}
+
+int setk_bss_eval(const float* est, const float* ref, const int32_t* n_samples_host, int32_t B, int32_t N, int32_t S,
+                  int32_t L, double* crit, int32_t* dropped, uint32_t* status, void* stream) {
+  if (!est || !ref || !crit || !status) return fail(SETK_EINVAL, "setk_bss_eval: null argument");
+  if (B < 1 || N < 1 || S < 1 || L < 1 || B > 65535)
+    return fail(SETK_EINVAL, "setk_bss_eval: bad shape B=%d N=%d S=%d L=%d", B, N, S, L);
+  if (N > SETK_SEP_MAX_SOURCES || L > SETK_SEP_MAX_FLEN || N * L > SETK_SEP_MAX_COLS || S > SETK_SEP_MAX_SAMPLES)
+    return fail(SETK_EUNSUPPORTED, "setk_bss_eval: N=%d L=%d S=%d: want N <= %d, L <= %d, N L <= %d, S <= %d", N, L, S,
+                SETK_SEP_MAX_SOURCES, SETK_SEP_MAX_FLEN, SETK_SEP_MAX_COLS, SETK_SEP_MAX_SAMPLES);
+  std::vector<int> len;
+  const int rc = sep_lengths("setk_bss_eval", n_samples_host, B, S, len);
+  if (rc != SETK_OK) return rc;
+  const size_t len_bytes = up256(sizeof(int) * B);
+  return with_scratch(bss_eval_scratch(B, N, S, L), stream, "setk_bss_eval(workspace)",
+                      "setk_bss_eval", [&](char* ws) {
+    cudaError_t e = cudaMemcpyAsync(ws, len.data(), sizeof(int) * B, cudaMemcpyHostToDevice,
+                                    static_cast<cudaStream_t>(stream));
+    if (e != cudaSuccess) return e;
+    return run_bss_eval(est, ref, reinterpret_cast<const int*>(ws), B, N, S, L, ws + len_bytes, crit, dropped,
+                        status, stream);
+  });
+}
+
+int setk_si_snr(const float* est, const float* ref, const int32_t* n_samples_host, int32_t B, int32_t N, int32_t S,
+                int32_t remove_dc, double eps, double* out, void* stream) {
+  if (!est || !ref || !out) return fail(SETK_EINVAL, "setk_si_snr: null argument");
+  if (B < 1 || N < 1 || S < 1 || B > 65535 || !(eps >= 0) || !std::isfinite(eps))
+    return fail(SETK_EINVAL, "setk_si_snr: bad argument B=%d N=%d S=%d eps=%g", B, N, S, eps);
+  if (N > SETK_SEP_MAX_SOURCES || S > SETK_SEP_MAX_SAMPLES)
+    return fail(SETK_EUNSUPPORTED, "setk_si_snr: N=%d S=%d: want N <= %d, S <= %d", N, S, SETK_SEP_MAX_SOURCES,
+                SETK_SEP_MAX_SAMPLES);
+  std::vector<int> len;
+  const int rc = sep_lengths("setk_si_snr", n_samples_host, B, S, len);
+  if (rc != SETK_OK) return rc;
+  return with_scratch(sizeof(int) * B, stream, "setk_si_snr(workspace)", "setk_si_snr", [&](char* ws) {
+    cudaError_t e = cudaMemcpyAsync(ws, len.data(), sizeof(int) * B, cudaMemcpyHostToDevice,
+                                    static_cast<cudaStream_t>(stream));
+    if (e != cudaSuccess) return e;
+    return run_si_snr(est, ref, reinterpret_cast<const int*>(ws), B, N, S, remove_dc, eps, out, stream);
+  });
+}
+
 }  // extern "C"

@@ -139,6 +139,13 @@ cudaError_t run_simulate_mix(const float* pool, int B, int n_terms, int M, int K
                              char* ws, const setk_simu_mix_t* mixes_host, const setk_simu_term_t* terms_host,
                              void* mix, void* spk, void* noise, double* factor, void* stream);
 
+// ---- sep_eval.cu: BSS-Eval and SI-SNR separation metrics ----
+size_t sep_eval_scratch_bytes(int B, int N, int S, int L);
+cudaError_t run_bss_eval(const float* est, const float* ref, const int* len, int B, int N, int S, int L, char* ws,
+                         double* crit, int* dropped, unsigned* status, void* stream);
+cudaError_t run_si_snr(const float* est, const float* ref, const int* len, int B, int N, int S, int remove_dc,
+                       double eps, double* out, void* stream);
+
 // ---- cm_mask.cu: Kaldi compressed-matrix masks ----
 cudaError_t run_cm_masks(const unsigned char* blobs, long long slot_bytes, int B, int T, int F, float* out,
                          int* status, void* stream);

@@ -831,3 +831,81 @@ def simulate_mix(pool, mixes, terms, n_channels, n_speakers, n_samples, pcm16=Fa
             M, K, N, int(bool(pcm16)), _lib.ptr(mix), _lib.ptr(s), _lib.ptr(nz), _lib.ptr(factor),
             _lib.current_stream(dev)))
     return mix, s, nz, factor
+
+
+# ---------------------------------------------------------------------------
+# Separation metrics (compute_sdr.py / compute_si_snr.py / libs/metric.py of the reference; csrc/sep_eval.cu)
+# ---------------------------------------------------------------------------
+SEP_SCRATCH_BYTES = 4 << 30   # bss_eval splits a batch so that one call's scratch stays under this (4 GiB)
+
+
+def _sep_inputs(est, ref, n_samples, who):
+    est, ref = torch.as_tensor(est), torch.as_tensor(ref)
+    if est.dim() != 3 or est.shape != ref.shape:
+        raise ValueError(f"{who}: est {tuple(est.shape)} and ref {tuple(ref.shape)} must both be (B, N, S)")
+    dev = ref.device if ref.device.type != "cpu" else est.device
+    est, ref = _f32(est, dev), _f32(ref, dev)
+    B, N, S = est.shape
+    lens = None
+    if n_samples is not None:
+        lens = np.ascontiguousarray(np.broadcast_to(np.asarray(n_samples, dtype=np.int64), (B,))).astype(np.int32)
+        if lens.size and (lens.min() < 1 or lens.max() > S):
+            raise ValueError(f"{who}: n_samples must lie in [1, {S}]")
+    return est, ref, lens, dev
+
+
+def _i32p(a):
+    return None if a is None else a.ctypes.data_as(ctypes.POINTER(ctypes.c_int32))
+
+
+def bss_eval_batch_step(B, N, S, flen=512):
+    """utterances per setk_bss_eval call that bss_eval uses for a (B, N, S) batch: all B when the call's
+    scratch (setk_bss_eval_scratch_bytes) fits SEP_SCRATCH_BYTES, else the most that fit (at least 1)"""
+    lib = _lib.library()
+    total = lib.setk_bss_eval_scratch_bytes(B, N, S, int(flen))
+    if total < 0 or total <= SEP_SCRATCH_BYTES:
+        return B   # sizes setk_bss_eval rejects are reported by the call itself
+    step = max(1, B * SEP_SCRATCH_BYTES // total)
+    while step > 1 and lib.setk_bss_eval_scratch_bytes(step, N, S, int(flen)) > SEP_SCRATCH_BYTES:
+        step -= 1
+    return step
+
+
+def bss_eval(est, ref, n_samples=None, flen=512):
+    """
+    BSS-Eval v3 sources criteria (mir_eval.separation.bss_eval_sources before its permutation search) of
+    every (estimate j, reference i) pair: est, ref (B, N, S) float32, n_samples (B,) true lengths of a
+    ragged batch (None: S), flen the filter length L.  Returns (crit (B, 3, N, N) float64 with
+    crit[b, k, j, i] the SDR / SIR / SAR (k = 0, 1, 2) of estimate j against reference i, dropped (B,)
+    int32 dependent columns of the least-squares system, status (B,) int32 SETK_ST_* bits).
+    """
+    est, ref, lens, dev = _sep_inputs(est, ref, n_samples, "bss_eval")
+    B, N, S = est.shape
+    L = int(flen)
+    crit = torch.empty((B, 3, N, N), dtype=torch.float64, device=dev)
+    dropped = torch.zeros((B,), dtype=torch.int32, device=dev)
+    status = torch.zeros((B,), dtype=torch.int32, device=dev)
+    step = bss_eval_batch_step(B, N, S, L)
+    with _ctx(dev):
+        for b0 in range(0, B, step):
+            b1 = min(B, b0 + step)
+            _lib.check(_lib.library().setk_bss_eval(
+                _lib.ptr(est[b0:b1]), _lib.ptr(ref[b0:b1]), _i32p(None if lens is None else lens[b0:b1]),
+                b1 - b0, N, S, L, _lib.ptr(crit[b0:b1]), _lib.ptr(dropped[b0:b1]), _lib.ptr(status[b0:b1]),
+                _lib.current_stream(dev)))
+    return crit, dropped, status
+
+
+def si_snr(est, ref, n_samples=None, remove_dc=True, eps=1e-8):
+    """
+    si_snr(x, s, eps, remove_dc) of libs/metric.py for every (estimate j, reference i) pair in fp64: est,
+    ref (B, N, S) float32, n_samples (B,) true lengths (None: S).  Returns (B, N, N) float64, [b, j, i].
+    """
+    est, ref, lens, dev = _sep_inputs(est, ref, n_samples, "si_snr")
+    B, N, S = est.shape
+    out = torch.empty((B, N, N), dtype=torch.float64, device=dev)
+    with _ctx(dev):
+        _lib.check(_lib.library().setk_si_snr(_lib.ptr(est), _lib.ptr(ref), _i32p(lens), B, N, S,
+                                              int(bool(remove_dc)), float(eps), _lib.ptr(out),
+                                              _lib.current_stream(dev)))
+    return out
