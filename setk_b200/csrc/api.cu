@@ -28,6 +28,8 @@ static int cuda_fail(cudaError_t e, const char* what) {
   snprintf(g_err, sizeof(g_err), "%s: CUDA error %d (%s)", what, (int)e, cudaGetErrorString(e));
   return (int)e;
 }
+// the return of every entry point: SETK_OK, or the CUDA error reported as `who`
+static int done(cudaError_t e, const char* who) { return e == cudaSuccess ? SETK_OK : cuda_fail(e, who); }
 
 // grow-only device workspace
 template <class T>
@@ -53,7 +55,7 @@ static int stft_to_bin_major(setk_plan* pl, const float* audio, const int32_t* n
   const int groups = (g.C + 3) / 4;   // the kernels take channels in groups of <= 4
   e = run_stft_spill(pl, audio, n_samples, B, N, T, stft_cov_pick_chunks(pl, B * groups, T), pl->d_stft_ws,
                      maxabs_bits, stream);
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, run_what);
+  return done(e, run_what);
 }
 
 // Runs run(scratch) with `bytes` of scratch allocated on the caller's stream (cudaMallocAsync /
@@ -68,7 +70,34 @@ static int with_scratch(size_t bytes, void* stream, const char* alloc_what, cons
   e = run(ws);
   const cudaError_t ef = cudaFreeAsync(ws, st);
   if (e == cudaSuccess) e = ef;
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, run_what);
+  return done(e, run_what);
+}
+
+// with_scratch with the host table `table` copied to its head on the stream (256-byte aligned): runs
+// run(device table, the `bytes` of scratch after it)
+template <class Run>
+static int with_host_table(const std::vector<int>& table, size_t bytes, void* stream, const char* alloc_what,
+                           const char* run_what, Run run) {
+  const size_t table_bytes = up256(sizeof(int) * table.size());
+  return with_scratch(table_bytes + bytes, stream, alloc_what, run_what, [&](char* ws) {
+    const cudaError_t e = cudaMemcpyAsync(ws, table.data(), sizeof(int) * table.size(), cudaMemcpyHostToDevice,
+                                          static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? run(reinterpret_cast<const int*>(ws), ws + table_bytes) : e;
+  });
+}
+
+// with_scratch holding the bin-major copy X [B][T][C][P = bin_pitch(F)] of a [B][C][F][T] STFT, then
+// (256-byte aligned) `bytes` of workspace: runs run(X, P, workspace) once the copy is enqueued
+template <class Run>
+static int with_bin_major(const void* stft, int B, int C, int F, int T, size_t bytes, void* stream,
+                          const char* alloc_what, const char* run_what, Run run) {
+  const int P = bin_pitch(F);
+  const size_t x_bytes = sizeof(float2) * (size_t)B * T * C * P;
+  return with_scratch(x_bytes + bytes + 256, stream, alloc_what, run_what, [&](char* ws) {
+    float2* X = reinterpret_cast<float2*>(ws);
+    const cudaError_t e = run_bcft_to_spill(static_cast<const float2*>(stft), B, C, F, T, P, X, stream);
+    return e == cudaSuccess ? run(X, P, reinterpret_cast<double*>(ws + up256(x_bytes))) : e;
+  });
 }
 
 }  // namespace setk
@@ -196,7 +225,7 @@ int setk_stft(setk_plan_t* pl, const float* audio, const int32_t* n_samples, int
   } else {
     e = run_stft_generic(pl, audio, n_samples, B, N, T, static_cast<float2*>(stft_out), stream);
   }
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_stft");
+  return done(e, "setk_stft");
 }
 
 int setk_cov(const void* stft, const float* mask, uint32_t flags, int32_t B, int32_t C, int32_t F,
@@ -207,7 +236,7 @@ int setk_cov(const void* stft, const float* mask, uint32_t flags, int32_t B, int
   if (B > 65535) return fail(SETK_ESHAPE, "setk_cov: batch %d > 65535", B);
   cudaError_t e = run_cov_generic(static_cast<const float2*>(stft), mask, flags, B, C, F, T,
                                   static_cast<float2*>(R), stream);
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_cov");
+  return done(e, "setk_cov");
 }
 
 int setk_stft_cov(setk_plan_t* pl, const float* audio, const int32_t* n_samples, int32_t B, int32_t N,
@@ -234,7 +263,7 @@ int setk_stft_cov(setk_plan_t* pl, const float* audio, const int32_t* n_samples,
     e = run_stft_cov_fused(pl, audio, n_samples, B, N, T, mask_s, mask_n, flags, pl->d_tile_prefix,
                            pl->d_partials, maxabs_bits, static_cast<float2*>(Rs),
                            static_cast<float2*>(Rn), maxabs, stream);
-    return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_stft_cov");
+    return done(e, "setk_stft_cov");
   }
   if (stft_spill_supported(g)) {
     // many-channel route (C > 4 at n_fft = 512, any C at n_fft = 1024): fast STFT
@@ -249,7 +278,7 @@ int setk_stft_cov(setk_plan_t* pl, const float* audio, const int32_t* n_samples,
     e = run_cov_spill(pl, pl->d_stft_ws, mask_s, mask_n, flags, n_samples, B, N, T, chunks, pl->d_partials,
                       static_cast<float2*>(Rs), static_cast<float2*>(Rn), stream);
     if (e == cudaSuccess && maxabs) e = run_bits_to_float(maxabs_bits, B, maxabs, stream);
-    return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_stft_cov(spill)");
+    return done(e, "setk_stft_cov(spill)");
   }
   // shape-generic route: explicit STFT in workspace, then two covariance passes
   const size_t want = sizeof(float2) * (size_t)B * g.C * g.F * T;
@@ -268,7 +297,7 @@ int setk_stft_cov(setk_plan_t* pl, const float* audio, const int32_t* n_samples,
   }
   if (e == cudaSuccess && maxabs)
     e = maxabs_generic(audio, n_samples, B, g.C, N, maxabs_bits, maxabs, stream);
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_stft_cov(generic)");
+  return done(e, "setk_stft_cov(generic)");
 }
 
 int setk_weights(int32_t kind, double beta, int32_t ref_channel, int32_t rank1, int32_t ban,
@@ -289,7 +318,7 @@ int setk_weights(int32_t kind, double beta, int32_t ref_channel, int32_t rank1, 
   if (rank1 < SETK_RANK1_NONE || rank1 > SETK_RANK1_GEV) return fail(SETK_EINVAL, "setk_weights: bad rank1 %d", rank1);
   cudaError_t e = weights_run(kind, beta, ref_channel, rank1, ban, Rs, Rn, Ry, r_dtype, B, F, C, w, w_dtype,
                               status, ref_used, stream);
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_weights");
+  return done(e, "setk_weights");
 }
 
 int setk_ban(const void* w_in, const void* Rn, int32_t dtype, int32_t B, int32_t F, int32_t C,
@@ -298,7 +327,7 @@ int setk_ban(const void* w_in, const void* Rn, int32_t dtype, int32_t B, int32_t
   if (B < 1 || F < 1 || C < 1 || C > SETK_MAX_CHANNELS) return fail(SETK_ESHAPE, "setk_ban: bad shape");
   if (dtype != SETK_C64 && dtype != SETK_C128) return fail(SETK_EINVAL, "setk_ban: bad dtype");
   cudaError_t e = post_run(0, w_in, Rn, dtype, B, F, C, w_out, nullptr, stream);
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_ban");
+  return done(e, "setk_ban");
 }
 
 int setk_rank1(const void* Rs, const void* Rn, int32_t dtype, int32_t B, int32_t F, int32_t C,
@@ -307,7 +336,7 @@ int setk_rank1(const void* Rs, const void* Rn, int32_t dtype, int32_t B, int32_t
   if (B < 1 || F < 1 || C < 1 || C > SETK_MAX_CHANNELS) return fail(SETK_ESHAPE, "setk_rank1: bad shape");
   if (dtype != SETK_C64 && dtype != SETK_C128) return fail(SETK_EINVAL, "setk_rank1: bad dtype");
   cudaError_t e = post_run(1, Rs, Rn, dtype, B, F, C, R1_out, status, stream);
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_rank1");
+  return done(e, "setk_rank1");
 }
 
 int setk_apply(const void* stft, const void* w, int32_t w_dtype, const float* post_mask, int32_t B,
@@ -317,7 +346,7 @@ int setk_apply(const void* stft, const void* w, int32_t w_dtype, const float* po
     return fail(SETK_ESHAPE, "setk_apply: bad shape B=%d C=%d F=%d T=%d", B, C, F, T);
   cudaError_t e = run_apply_generic(static_cast<const float2*>(stft), w, w_dtype, post_mask, B, C, F, T,
                                     static_cast<float2*>(enh), stream);
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_apply");
+  return done(e, "setk_apply");
 }
 
 int setk_istft(setk_plan_t* pl, const void* enh, int32_t B, int32_t T, int32_t n_out, const float* norm,
@@ -338,7 +367,7 @@ int setk_istft(setk_plan_t* pl, const void* enh, int32_t B, int32_t T, int32_t n
   e = run_istft_generic(pl, static_cast<const float2*>(enh), B, T, T_used, n_out, nullptr, pl->d_frames_ws,
                         wave, peak, stream);
   if (e == cudaSuccess && norm) e = run_peak_scale(wave, B, n_out, norm, peak, stream);
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_istft");
+  return done(e, "setk_istft");
 }
 
 // wave != null: float output (+ norm rescale in place); pcm != null: the float wave goes to a plan
@@ -398,7 +427,7 @@ static int apply_istft_impl(setk_plan_t* pl, const float* audio, const int32_t* 
   }
   if (e == cudaSuccess && pcm) e = run_peak_scale_pcm16(wave, B, n_out, norm, peak, pcm, stream);
   else if (e == cudaSuccess && norm) e = run_peak_scale(wave, B, n_out, norm, peak, stream);
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_apply_istft");
+  return done(e, "setk_apply_istft");
 }
 
 int setk_apply_istft(setk_plan_t* pl, const float* audio, const int32_t* n_samples, int32_t B, int32_t N,
@@ -444,7 +473,7 @@ int setk_cgmm_masks(setk_plan_t* pl, const float* audio, const int32_t* n_sample
   if (rc) return rc;
   e = run_cgmm(&ctx, pl->d_stft_ws, P, pl->d_cgmm_ws, n_samples, B, N, T, num_classes, num_iters, init_gamma,
                update_alpha, masks, status, stream);
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_cgmm_masks");
+  return done(e, "setk_cgmm_masks");
 }
 
 int setk_cgmm_stft(const void* stft, int32_t B, int32_t C, int32_t F, int32_t T, int32_t num_classes,
@@ -466,18 +495,10 @@ int setk_cgmm_stft(const void* stft, int32_t B, int32_t C, int32_t F, int32_t T,
   cudaError_t e = cudaGetDevice(&dev);
   if (e == cudaSuccess) e = cudaDeviceGetAttribute(&ctx.sm_count, cudaDevAttrMultiProcessorCount, dev);
   if (e != cudaSuccess) return cuda_fail(e, "setk_cgmm_stft(device)");
-  // scratch: the bin-major copy X of the STFT, then (256-byte aligned) the CGMM workspace
-  const int P = bin_pitch(F);
-  const size_t x_bytes = sizeof(float2) * (size_t)B * T * C * P;
-  const size_t w_bytes = cgmm_workspace_bytes(&ctx, B, T, num_classes, P);
-  return with_scratch(x_bytes + w_bytes + 256, stream, "setk_cgmm_stft(workspace)", "setk_cgmm_stft",
-                      [&](char* ws) {
-    float2* X = reinterpret_cast<float2*>(ws);
-    cudaError_t e = run_bcft_to_spill(static_cast<const float2*>(stft), B, C, F, T, P, X, stream);
-    if (e == cudaSuccess)
-      e = run_cgmm(&ctx, X, P, reinterpret_cast<double*>(ws + up256(x_bytes)), nullptr, B, /*N=*/T + 1, T,
-                   num_classes, num_iters, init_gamma, update_alpha, masks, status, stream);
-    return e;
+  return with_bin_major(stft, B, C, F, T, cgmm_workspace_bytes(&ctx, B, T, num_classes, bin_pitch(F)), stream,
+                        "setk_cgmm_stft(workspace)", "setk_cgmm_stft", [&](float2* X, int P, double* ws) {
+    return run_cgmm(&ctx, X, P, ws, nullptr, B, /*N=*/T + 1, T, num_classes, num_iters, init_gamma, update_alpha,
+                    masks, status, stream);
   });
 }
 
@@ -493,17 +514,10 @@ static int wpe_entry(const char* who, const void* stft, const void* lambda_enh, 
   if (!wpe_supported(C, T, taps, delay, context))
     return fail(SETK_EUNSUPPORTED, "%s: %d channels x %d taps (context %d) exceeds the kernels' "
                 "shared-memory budget", who, C, taps, context);
-  // scratch: the bin-major copy X of the STFT, then (256-byte aligned) the WPE workspace
-  const int P = bin_pitch(F);
-  const size_t x_bytes = sizeof(float2) * (size_t)B * T * C * P;
-  const size_t w_bytes = wpe_workspace_bytes(B, C, F, taps);
-  return with_scratch(x_bytes + w_bytes + 256, stream, who, who, [&](char* ws) {
-    float2* X = reinterpret_cast<float2*>(ws);
-    cudaError_t e = run_bcft_to_spill(static_cast<const float2*>(stft), B, C, F, T, P, X, stream);
-    if (e == cudaSuccess)
-      e = run_wpe(X, P, B, C, F, T, taps, delay, context, num_iters, reinterpret_cast<double*>(ws + up256(x_bytes)),
-                  static_cast<float2*>(out), status, static_cast<const float2*>(lambda_enh), inv_lambda, stream);
-    return e;
+  return with_bin_major(stft, B, C, F, T, wpe_workspace_bytes(B, C, F, taps), stream, who, who,
+                        [&](float2* X, int P, double* ws) {
+    return run_wpe(X, P, B, C, F, T, taps, delay, context, num_iters, ws, static_cast<float2*>(out), status,
+                   static_cast<const float2*>(lambda_enh), inv_lambda, stream);
   });
 }
 
@@ -524,14 +538,14 @@ int setk_float_to_pcm16(const float* wave, int64_t n, int16_t* pcm, void* stream
   if (!wave || !pcm || n < 0) return fail(SETK_EINVAL, "setk_float_to_pcm16: bad argument");
   if (n == 0) return SETK_OK;
   cudaError_t e = run_float_to_pcm16(wave, n, pcm, stream);
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_float_to_pcm16");
+  return done(e, "setk_float_to_pcm16");
 }
 
 int setk_pcm16_to_float(const int16_t* pcm, int64_t n, float* wave, void* stream) {
   if (!wave || !pcm || n < 0) return fail(SETK_EINVAL, "setk_pcm16_to_float: bad argument");
   if (n == 0) return SETK_OK;
   cudaError_t e = run_pcm16_to_float(pcm, n, wave, stream);
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_pcm16_to_float");
+  return done(e, "setk_pcm16_to_float");
 }
 
 int setk_cm_masks(const uint8_t* blobs, int64_t slot_bytes, int32_t B, int32_t T, int32_t F, float* out,
@@ -540,7 +554,7 @@ int setk_cm_masks(const uint8_t* blobs, int64_t slot_bytes, int32_t B, int32_t T
       (reinterpret_cast<uintptr_t>(blobs) & 15))
     return fail(SETK_EINVAL, "setk_cm_masks: bad argument");
   cudaError_t e = run_cm_masks(blobs, slot_bytes, B, T, F, out, status, stream);
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_cm_masks");
+  return done(e, "setk_cm_masks");
 }
 
 // ---- spatial features (spatial.cu) ----
@@ -551,7 +565,7 @@ int setk_ipd(const void* si, const void* sj, int64_t rows, int32_t F, int32_t mo
   if (mode < 0 || mode > 2) return fail(SETK_EINVAL, "setk_ipd: mode %d outside 0..2", mode);
   cudaError_t e = run_ipd(static_cast<const float2*>(si), static_cast<const float2*>(sj), rows, F, mode,
                           out, stream);
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_ipd");
+  return done(e, "setk_ipd");
 }
 
 int setk_directional_feats(const void* stft, const void* steer, int32_t steer_batched,
@@ -563,7 +577,7 @@ int setk_directional_feats(const void* stft, const void* steer, int32_t steer_ba
   if (pairs && n_pairs < 1) return fail(SETK_EINVAL, "setk_directional_feats: empty pair list");
   cudaError_t e = run_dirfeat(static_cast<const float2*>(stft), static_cast<const double2*>(steer),
                               steer_batched, pairs, n_pairs, B, M, F, T, out, stream);
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_directional_feats");
+  return done(e, "setk_directional_feats");
 }
 
 int64_t setk_gcc_phat_work_doubles(int32_t T, int32_t F, int32_t D) {
@@ -580,7 +594,7 @@ int setk_gcc_phat(const void* si, const void* sj, int32_t T, int32_t F, const do
     return fail(SETK_EUNSUPPORTED, "setk_gcc_phat: F=%d too large (<= 3072 bins)", F);
   cudaError_t e = run_gcc_phat(static_cast<const float2*>(si), static_cast<const float2*>(sj), T, F, omega,
                                tau, D, normalize, apply_floor, accumulate, work, out, stream);
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_gcc_phat");
+  return done(e, "setk_gcc_phat");
 }
 
 int64_t setk_msc_work_doubles(int32_t T, int32_t F) {
@@ -595,7 +609,7 @@ int setk_msc(const void* spec, int32_t N, int32_t T, int32_t F, int32_t context,
     return fail(SETK_ESHAPE, "setk_msc: bad shape N=%d T=%d F=%d", N, T, F);
   if (context < 0) return fail(SETK_EINVAL, "setk_msc: context %d < 0", context);
   cudaError_t e = run_msc(static_cast<const float2*>(spec), N, T, F, context, normalize, work, out, stream);
-  return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_msc");
+  return done(e, "setk_msc");
 }
 
 // ---- sound source localisation (ssl.cuh, built in spatial.cu) ----
@@ -669,7 +683,7 @@ int setk_ns_imcra(const setk_imcra_config_t* cfg, const void* stft, const int32_
   const size_t ring = ns_ring_bytes(*cfg, B, F);
   if (ring == 0) {
     cudaError_t e = run_ns_imcra(*cfg, X, n_frames, B, F, T, nullptr, gain, out, stream);
-    return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_ns_imcra");
+    return done(e, "setk_ns_imcra");
   }
   return with_scratch(ring, stream, "setk_ns_imcra(workspace)", "setk_ns_imcra", [&](char* ws) {
     return run_ns_imcra(*cfg, X, n_frames, B, F, T, reinterpret_cast<double*>(ws), gain, out, stream);
@@ -718,7 +732,7 @@ int setk_rir_image(const setk_rir_config_t* cfg, const double* room, const doubl
   }
   if (rir_segments(L) == 1 || !cfg->hp_filter) {
     e = run_rir_image(*cfg, room, beta, source, receivers, B, M, max_n, rir, nullptr, status, stream);
-    return e == cudaSuccess ? SETK_OK : cuda_fail(e, "setk_rir_image");
+    return done(e, "setk_rir_image");
   }
   return with_scratch(sizeof(double) * (size_t)B * M * L, stream, "setk_rir_image(workspace)", "setk_rir_image",
                       [&](char* ws) {
@@ -748,13 +762,9 @@ int setk_convolve(const float* x, int32_t Sx, const float* h, int32_t Lh, int32_
     len[3 * (size_t)b + 1] = L;
     len[3 * (size_t)b + 2] = n;
   }
-  const size_t len_bytes = up256(sizeof(int) * len.size());
-  return with_scratch(len_bytes + conv_spectra_bytes(B, M, Lh, Ny), stream, "setk_convolve(workspace)",
-                      "setk_convolve", [&](char* ws) {
-    cudaError_t e = cudaMemcpyAsync(ws, len.data(), sizeof(int) * len.size(), cudaMemcpyHostToDevice,
-                                    static_cast<cudaStream_t>(stream));
-    if (e != cudaSuccess) return e;
-    return run_convolve(x, Sx, h, Lh, B, M, reinterpret_cast<const int*>(ws), y, Ny, ws + len_bytes, stream);
+  return with_host_table(len, conv_spectra_bytes(B, M, Lh, Ny), stream, "setk_convolve(workspace)", "setk_convolve",
+                         [&](const int* d_len, char* ws) {
+    return run_convolve(x, Sx, h, Lh, B, M, d_len, y, Ny, ws, stream);
   });
 }
 
@@ -818,15 +828,12 @@ static int sep_lengths(const char* who, const int32_t* n_samples_host, int B, in
   return SETK_OK;
 }
 
-static size_t bss_eval_scratch(int B, int N, int S, int L) {
-  return up256(sizeof(int) * B) + sep_eval_scratch_bytes(B, N, S, L);
-}
-
 int64_t setk_bss_eval_scratch_bytes(int32_t B, int32_t N, int32_t S, int32_t L) {
   if (B < 1 || N < 1 || S < 1 || L < 1 || B > 65535 || N > SETK_SEP_MAX_SOURCES || L > SETK_SEP_MAX_FLEN ||
       N * L > SETK_SEP_MAX_COLS || S > SETK_SEP_MAX_SAMPLES)
     return -1;
-  return (int64_t)bss_eval_scratch(B, N, S, L);
+  // what setk_bss_eval's with_host_table allocates: the B lengths, then the kernels' scratch
+  return (int64_t)(up256(sizeof(int) * B) + sep_eval_scratch_bytes(B, N, S, L));
 }
 
 int setk_bss_eval(const float* est, const float* ref, const int32_t* n_samples_host, int32_t B, int32_t N, int32_t S,
@@ -840,14 +847,9 @@ int setk_bss_eval(const float* est, const float* ref, const int32_t* n_samples_h
   std::vector<int> len;
   const int rc = sep_lengths("setk_bss_eval", n_samples_host, B, S, len);
   if (rc != SETK_OK) return rc;
-  const size_t len_bytes = up256(sizeof(int) * B);
-  return with_scratch(bss_eval_scratch(B, N, S, L), stream, "setk_bss_eval(workspace)",
-                      "setk_bss_eval", [&](char* ws) {
-    cudaError_t e = cudaMemcpyAsync(ws, len.data(), sizeof(int) * B, cudaMemcpyHostToDevice,
-                                    static_cast<cudaStream_t>(stream));
-    if (e != cudaSuccess) return e;
-    return run_bss_eval(est, ref, reinterpret_cast<const int*>(ws), B, N, S, L, ws + len_bytes, crit, dropped,
-                        status, stream);
+  return with_host_table(len, sep_eval_scratch_bytes(B, N, S, L), stream, "setk_bss_eval(workspace)", "setk_bss_eval",
+                         [&](const int* d_len, char* ws) {
+    return run_bss_eval(est, ref, d_len, B, N, S, L, ws, crit, dropped, status, stream);
   });
 }
 
@@ -862,11 +864,8 @@ int setk_si_snr(const float* est, const float* ref, const int32_t* n_samples_hos
   std::vector<int> len;
   const int rc = sep_lengths("setk_si_snr", n_samples_host, B, S, len);
   if (rc != SETK_OK) return rc;
-  return with_scratch(sizeof(int) * B, stream, "setk_si_snr(workspace)", "setk_si_snr", [&](char* ws) {
-    cudaError_t e = cudaMemcpyAsync(ws, len.data(), sizeof(int) * B, cudaMemcpyHostToDevice,
-                                    static_cast<cudaStream_t>(stream));
-    if (e != cudaSuccess) return e;
-    return run_si_snr(est, ref, reinterpret_cast<const int*>(ws), B, N, S, remove_dc, eps, out, stream);
+  return with_host_table(len, 0, stream, "setk_si_snr(workspace)", "setk_si_snr", [&](const int* d_len, char*) {
+    return run_si_snr(est, ref, d_len, B, N, S, remove_dc, eps, out, stream);
   });
 }
 

@@ -89,13 +89,7 @@ def _solve_dtype(*mats):
 def _weights(kind, Rs, Rn=None, Ry=None, **kw):
     Rs, was_np = _complex(Rs)
     Rs, squeeze = _batched(Rs, 3)
-    mats = [Rs]
-    for m in (Rn, Ry):
-        if m is None:
-            mats.append(None)
-        else:
-            t, _ = _complex(m)
-            mats.append(_batched(t.to(Rs.device), 3)[0])
+    mats = [Rs] + [None if m is None else _batched(_complex(m)[0], 3)[0] for m in (Rn, Ry)]
     dt = _solve_dtype(*mats)
     mats = [None if m is None else m.to(dt) for m in mats]
     w, status, ref = _plan.weights(kind, mats[0], mats[1], mats[2], out_dtype=dt, **kw)
@@ -111,7 +105,7 @@ def do_ban(weight, Rn):
     w, was_np = _complex(weight)
     w, squeeze = _batched(w, 2)
     R, _ = _complex(Rn)
-    R = _batched(R.to(w.device), 3)[0]
+    R = _batched(R, 3)[0]
     dt = _solve_dtype(w, R)
     out = _plan.ban(w.to(dt), R.to(dt))
     return _back(out[0] if squeeze else out, was_np)
@@ -134,7 +128,7 @@ def rank1_constraint(Rs, Rn=None):
     Rn_t = None
     if Rn is not None:
         Rn_t, _ = _complex(Rn)
-        Rn_t = _batched(Rn_t.to(R.device), 3)[0]
+        Rn_t = _batched(Rn_t, 3)[0]
     dt = _solve_dtype(R, Rn_t)
     out, status = _plan.rank1(R.to(dt), None if Rn_t is None else Rn_t.to(dt))
     _check_status(status)
@@ -149,7 +143,7 @@ def compute_covar(obs, tf_mask):
     x, was_np = _complex(obs)
     x, squeeze = _batched(x, 3)
     m, _ = _to_tensor(tf_mask, torch.float32)
-    m = _batched(m.to(x.device), 2)[0]
+    m = _batched(m, 2)[0]
     R = _plan.covariance(x, m)
     return _back(R[0] if squeeze else R, was_np)
 
@@ -166,7 +160,6 @@ class Beamformer(object):
         """
         x, was_np = _complex(obs)
         w, _ = _complex(weight)
-        w = w.to(x.device)
         x, squeeze = _batched(x, 3)
         w = _batched(w, 2)[0]
         if w.shape[-2] != x.shape[-2] or w.shape[-1] != x.shape[-3]:

@@ -8,6 +8,7 @@ Layouts are the reference's (scripts/sptk/libs): audio (B,C,N) f32, mask
 (B,T,F) f32, stft (B,C,F,T) c64, R (B,F,C,C), weight (B,F,C), enhanced
 (B,F,T) c64, wave (B,N_out) f32.
 """
+import contextlib
 import ctypes
 import math
 
@@ -51,11 +52,50 @@ def _dtype_code(t):
     raise TypeError(f"expected a complex64/complex128 tensor, got {t.dtype}")
 
 
-def _f32(t, device):
-    t = torch.as_tensor(t, device=device)
-    if t.dtype != torch.float32:
-        t = t.to(torch.float32)
-    return t.contiguous()
+def _arg(t, dev, dtype, shape, what):
+    """
+    A tensor input of a C-ABI call: `t` as a contiguous tensor on `dev` (None: where it is) of `dtype`
+    (None: its own), or None for None.  `shape` None takes any shape; else every entry that is not None
+    must match, or ValueError names `what`.  Reads metadata only, so it never synchronises the host.
+    """
+    if t is None:
+        return None
+    t = torch.as_tensor(t, dtype=dtype, device=dev).contiguous()
+    if shape is not None and (t.dim() != len(shape) or any(s is not None and s != n for s, n in zip(shape, t.shape))):
+        want = ", ".join("*" if s is None else str(s) for s in shape)
+        raise ValueError(f"{what} must be ({want}), got {tuple(t.shape)}")
+    return t
+
+
+def _out(t, dev, dtype, shape, what):
+    """A caller's output buffer: the kernel writes it in place, so it is never converted and must already
+    be a contiguous `dtype` tensor of `shape` on `dev` (ValueError naming `what` otherwise)."""
+    if t.dtype != dtype or tuple(t.shape) != tuple(shape) or t.device != dev or not t.is_contiguous():
+        raise ValueError(f"{what} must be a contiguous {dtype} {tuple(shape)} tensor on {dev}, got {t.dtype} "
+                         f"{tuple(t.shape)} on {t.device}, contiguous={t.is_contiguous()}")
+    return t
+
+
+def _host_i32(v, shape=None):
+    """
+    A host table for a C-ABI `const int32_t*` argument: (v as a C-contiguous int32 array, broadcast to
+    `shape` when given; the pointer the call takes, which keeps the array alive), or (None, None) for None.
+    """
+    if v is None:
+        return None, None
+    a = np.asarray(v, dtype=np.int32)
+    a = np.ascontiguousarray(a if shape is None else np.broadcast_to(a, shape))
+    return a, a.ctypes.data_as(ctypes.POINTER(ctypes.c_int32))
+
+
+def _ctx(device):
+    return torch.cuda.device(device) if device.type == "cuda" else contextlib.nullcontext()
+
+
+def _launch(dev, name, *args):
+    """libsetk_b200's `name`(*args, stream) on `dev`, on the current stream of `dev`; raises on an error."""
+    with _ctx(dev):
+        _lib.check(getattr(_lib.library(), name)(*args, _lib.current_stream(dev)))
 
 
 class StftPlan(object):
@@ -87,21 +127,15 @@ class StftPlan(object):
             max_batch=self.max_batch, max_samples=self.max_samples, reserved=0,
             window_host=self._win.ctypes.data_as(ctypes.POINTER(ctypes.c_double)))
         handle = ctypes.c_void_p()
-        with self._device_ctx():
+        with _ctx(self.device):
             _lib.check(_lib.library().setk_plan_create(ctypes.byref(cfg), ctypes.byref(handle)))
         self._h = handle
 
     # ------------------------------------------------------------------ misc
-    def _device_ctx(self):
-        if self.device.type == "cuda":
-            return torch.cuda.device(self.device)
-        import contextlib
-        return contextlib.nullcontext()
-
     def close(self):
         if getattr(self, "_h", None):
             try:
-                with self._device_ctx():
+                with _ctx(self.device):
                     _lib.library().setk_plan_destroy(self._h)
             finally:
                 self._h = None
@@ -121,22 +155,8 @@ class StftPlan(object):
     def istft_length(self, num_frames):
         return _lib.library().setk_istft_length(self._h, int(num_frames))
 
-    def _stream(self):
-        return _lib.current_stream(self.device)
-
     def _check_audio(self, audio):
-        audio = _f32(audio, self.device)
-        if audio.dim() != 3 or audio.shape[1] != self.num_channels:
-            raise ValueError(f"audio must be (B, {self.num_channels}, N), got {tuple(audio.shape)}")
-        return audio
-
-    def _nsamp(self, n_samples, B):
-        if n_samples is None:
-            return None
-        ns = torch.as_tensor(n_samples, device=self.device).to(torch.int32).contiguous()
-        if ns.shape != (B,):
-            raise ValueError(f"n_samples must have shape ({B},)")
-        return ns
+        return _arg(audio, self.device, torch.float32, (None, self.num_channels, None), "audio")
 
     # --------------------------------------------------------------- kernels
     def stft(self, audio, n_samples=None):
@@ -144,11 +164,9 @@ class StftPlan(object):
         audio = self._check_audio(audio)
         B, C, N = audio.shape
         T = self.num_frames(N)
-        ns = self._nsamp(n_samples, B)
+        ns = _arg(n_samples, self.device, torch.int32, (B,), "n_samples")
         out = torch.empty((B, C, self.num_bins, T), dtype=torch.complex64, device=self.device)
-        with self._device_ctx():
-            _lib.check(_lib.library().setk_stft(self._h, _lib.ptr(audio), _lib.ptr(ns), B, N,
-                                                _lib.ptr(out), self._stream()))
+        _launch(self.device, "setk_stft", self._h, _lib.ptr(audio), _lib.ptr(ns), B, N, _lib.ptr(out))
         return out
 
     def stft_cov(self, audio, mask_s, mask_n=None, n_samples=None, clip_mask=False,
@@ -162,22 +180,15 @@ class StftPlan(object):
         T = self.num_frames(N)
         F = self.num_bins
         mshape = (B, F, T) if mask_ft else (B, T, F)
-        mask_s = _f32(mask_s, self.device)
-        if tuple(mask_s.shape) != mshape:
-            raise ValueError(f"mask must be {mshape}, got {tuple(mask_s.shape)}")
-        if mask_n is not None:
-            mask_n = _f32(mask_n, self.device)
-            if tuple(mask_n.shape) != mshape:
-                raise ValueError(f"mask_n must be {mshape}, got {tuple(mask_n.shape)}")
-        ns = self._nsamp(n_samples, B)
+        mask_s = _arg(mask_s, self.device, torch.float32, mshape, "mask")
+        mask_n = _arg(mask_n, self.device, torch.float32, mshape, "mask_n")
+        ns = _arg(n_samples, self.device, torch.int32, (B,), "n_samples")
         Rs = torch.empty((B, F, C, C), dtype=torch.complex64, device=self.device)
         Rn = torch.empty_like(Rs)
         maxabs = torch.empty((B,), dtype=torch.float32, device=self.device) if want_maxabs else None
         flags = (_lib.F_CLIP_MASK if clip_mask else 0) | (_lib.F_MASK_FT if mask_ft else 0)
-        with self._device_ctx():
-            _lib.check(_lib.library().setk_stft_cov(
-                self._h, _lib.ptr(audio), _lib.ptr(ns), B, N, _lib.ptr(mask_s), _lib.ptr(mask_n),
-                flags, _lib.ptr(Rs), _lib.ptr(Rn), _lib.ptr(maxabs), self._stream()))
+        _launch(self.device, "setk_stft_cov", self._h, _lib.ptr(audio), _lib.ptr(ns), B, N, _lib.ptr(mask_s),
+                _lib.ptr(mask_n), flags, _lib.ptr(Rs), _lib.ptr(Rn), _lib.ptr(maxabs))
         return Rs, Rn, maxabs
 
     def cgmm_masks(self, audio, num_classes=2, num_iters=20, init_gamma=None, update_alpha=False,
@@ -192,35 +203,23 @@ class StftPlan(object):
         T = self.num_frames(N)
         F = self.num_bins
         K = int(num_classes)
-        if init_gamma is not None:
-            init_gamma = _f32(init_gamma, self.device)
-            if tuple(init_gamma.shape) != (B, K, T, F):
-                raise ValueError(f"init_gamma must be {(B, K, T, F)}, got {tuple(init_gamma.shape)}")
-        ns = self._nsamp(n_samples, B)
+        init_gamma = _arg(init_gamma, self.device, torch.float32, (B, K, T, F), "init_gamma")
+        ns = _arg(n_samples, self.device, torch.int32, (B,), "n_samples")
         masks = torch.empty((B, K, T, F), dtype=torch.float32, device=self.device)
         status = torch.zeros((B,), dtype=torch.int32, device=self.device)
-        with self._device_ctx():
-            _lib.check(_lib.library().setk_cgmm_masks(
-                self._h, _lib.ptr(audio), _lib.ptr(ns), B, N, K, int(num_iters), _lib.ptr(init_gamma),
-                1 if update_alpha else 0, _lib.ptr(masks), _lib.ptr(status), self._stream()))
+        _launch(self.device, "setk_cgmm_masks", self._h, _lib.ptr(audio), _lib.ptr(ns), B, N, K, int(num_iters),
+                _lib.ptr(init_gamma), 1 if update_alpha else 0, _lib.ptr(masks), _lib.ptr(status))
         return masks, status
 
     def istft(self, enh, n_out=None, norm=None):
         """enh (B,F,T) complex64 -> wave (B,n_out) float32 (inverse_stft)."""
-        enh = torch.as_tensor(enh, device=self.device)
-        if enh.dtype != torch.complex64:
-            enh = enh.to(torch.complex64)
-        enh = enh.contiguous()
-        if enh.dim() != 3 or enh.shape[1] != self.num_bins:
-            raise ValueError(f"enh must be (B, {self.num_bins}, T), got {tuple(enh.shape)}")
+        enh = _arg(enh, self.device, torch.complex64, (None, self.num_bins, None), "enh")
         B, F, T = enh.shape
         if n_out is None:
             n_out = self.istft_length(T)
-        norm_t = None if norm is None else _f32(norm, self.device).reshape(B)
+        norm = _arg(norm, self.device, torch.float32, (B,), "norm")
         wave = torch.empty((B, int(n_out)), dtype=torch.float32, device=self.device)
-        with self._device_ctx():
-            _lib.check(_lib.library().setk_istft(self._h, _lib.ptr(enh), B, T, int(n_out),
-                                                 _lib.ptr(norm_t), _lib.ptr(wave), self._stream()))
+        _launch(self.device, "setk_istft", self._h, _lib.ptr(enh), B, T, int(n_out), _lib.ptr(norm), _lib.ptr(wave))
         return wave
 
     def apply_istft(self, audio, weight, post_mask=None, n_out=None, norm=None, n_samples=None,
@@ -231,58 +230,36 @@ class StftPlan(object):
         audio = self._check_audio(audio)
         B, C, N = audio.shape
         T = self.num_frames(N)
-        weight = torch.as_tensor(weight, device=self.device).contiguous()
-        if tuple(weight.shape) != (B, self.num_bins, C):
-            raise ValueError(f"weight must be {(B, self.num_bins, C)}, got {tuple(weight.shape)}")
-        if post_mask is not None:
-            post_mask = _f32(post_mask, self.device)
-            if tuple(post_mask.shape) != (B, T, self.num_bins):
-                raise ValueError("post_mask must be (B, T, F)")
+        F = self.num_bins
+        weight = _arg(weight, self.device, None, (B, F, C), "weight")
+        post_mask = _arg(post_mask, self.device, torch.float32, (B, T, F), "post_mask")
         if n_out is None:
             n_out = self.istft_length(T)
-        norm_t = None if norm is None else _f32(norm, self.device).reshape(B)
-        ns = self._nsamp(n_samples, B)
+        norm = _arg(norm, self.device, torch.float32, (B,), "norm")
+        ns = _arg(n_samples, self.device, torch.int32, (B,), "n_samples")
         wave = torch.empty((B, int(n_out)), dtype=torch.int16 if pcm16 else torch.float32,
                            device=self.device)
-        fn = _lib.library().setk_apply_istft_pcm16 if pcm16 else _lib.library().setk_apply_istft
-        with self._device_ctx():
-            _lib.check(fn(
-                self._h, _lib.ptr(audio), _lib.ptr(ns), B, N, _lib.ptr(weight), _dtype_code(weight),
-                _lib.ptr(post_mask), int(n_out), _lib.ptr(norm_t), _lib.ptr(wave), self._stream()))
+        _launch(self.device, "setk_apply_istft_pcm16" if pcm16 else "setk_apply_istft", self._h, _lib.ptr(audio),
+                _lib.ptr(ns), B, N, _lib.ptr(weight), _dtype_code(weight), _lib.ptr(post_mask), int(n_out),
+                _lib.ptr(norm), _lib.ptr(wave))
         return wave
 
 
 # ---------------------------------------------------------------- plan-free ---
-def _ctx(device):
-    if device.type == "cuda":
-        return torch.cuda.device(device)
-    import contextlib
-    return contextlib.nullcontext()
-
-
 def cgmm_from_stft(stft, num_classes=2, num_iters=20, init_gamma=None, update_alpha=False):
     """
     CgmmTrainer(obs, K, gamma, update_alpha).train(num_iters) batched (cluster.py:396-465).
     stft (B,C,F,T) complex64; init_gamma (B,K,T,F) or None (2 classes only).
     Returns (masks (B,K,T,F) float32, status (B,) int32).
     """
-    stft = stft.contiguous()
-    if stft.dtype != torch.complex64:
-        stft = stft.to(torch.complex64)
-    if stft.dim() != 4:
-        raise ValueError(f"stft must be (B, C, F, T), got {tuple(stft.shape)}")
+    stft = _arg(stft, None, torch.complex64, (None,) * 4, "stft")
     B, C, F, T = stft.shape
     K = int(num_classes)
-    if init_gamma is not None:
-        init_gamma = _f32(init_gamma, stft.device)
-        if tuple(init_gamma.shape) != (B, K, T, F):
-            raise ValueError(f"init_gamma must be {(B, K, T, F)}, got {tuple(init_gamma.shape)}")
+    init_gamma = _arg(init_gamma, stft.device, torch.float32, (B, K, T, F), "init_gamma")
     masks = torch.empty((B, K, T, F), dtype=torch.float32, device=stft.device)
     status = torch.zeros((B,), dtype=torch.int32, device=stft.device)
-    with _ctx(stft.device):
-        _lib.check(_lib.library().setk_cgmm_stft(
-            _lib.ptr(stft), B, C, F, T, K, int(num_iters), _lib.ptr(init_gamma), 1 if update_alpha else 0,
-            _lib.ptr(masks), _lib.ptr(status), _lib.current_stream(stft.device)))
+    _launch(stft.device, "setk_cgmm_stft", _lib.ptr(stft), B, C, F, T, K, int(num_iters), _lib.ptr(init_gamma),
+            1 if update_alpha else 0, _lib.ptr(masks), _lib.ptr(status))
     return masks, status
 
 
@@ -291,18 +268,12 @@ def wpe_from_stft(stft, taps=10, delay=3, context=1, num_iters=3):
     wpe(reverb, taps, delay, context, num_iters) batched (libs/wpe.py:82-110).
     stft (B,C,F,T) complex64 -> (dereverberated (B,C,F,T) complex64, status (B,) int32).
     """
-    stft = stft.contiguous()
-    if stft.dtype != torch.complex64:
-        stft = stft.to(torch.complex64)
-    if stft.dim() != 4:
-        raise ValueError(f"stft must be (B, C, F, T), got {tuple(stft.shape)}")
+    stft = _arg(stft, None, torch.complex64, (None,) * 4, "stft")
     B, C, F, T = stft.shape
     out = torch.empty_like(stft)
     status = torch.zeros((B,), dtype=torch.int32, device=stft.device)
-    with _ctx(stft.device):
-        _lib.check(_lib.library().setk_wpe_stft(
-            _lib.ptr(stft), B, C, F, T, int(taps), int(delay), int(context), int(num_iters),
-            _lib.ptr(out), _lib.ptr(status), _lib.current_stream(stft.device)))
+    _launch(stft.device, "setk_wpe_stft", _lib.ptr(stft), B, C, F, T, int(taps), int(delay), int(context),
+            int(num_iters), _lib.ptr(out), _lib.ptr(status))
     return out, status
 
 
@@ -312,39 +283,34 @@ def wpe_step(stft, lambda_enh=None, taps=10, delay=3, context=1, want_inv_lambda
     lambda_enh (B,F,T) complex64 or None (first iteration: compute_lambda of the observations).
     Returns (dereverberated (B,C,F,T) complex64, 1/lambda (B,T,F) float32 or None, status (B,) int32).
     """
-    stft = stft.contiguous()
-    if stft.dtype != torch.complex64:
-        stft = stft.to(torch.complex64)
-    if stft.dim() != 4:
-        raise ValueError(f"stft must be (B, C, F, T), got {tuple(stft.shape)}")
+    stft = _arg(stft, None, torch.complex64, (None,) * 4, "stft")
     B, C, F, T = stft.shape
-    if lambda_enh is not None:
-        lambda_enh = torch.as_tensor(lambda_enh, device=stft.device).to(torch.complex64).contiguous()
-        if tuple(lambda_enh.shape) != (B, F, T):
-            raise ValueError(f"lambda_enh must be {(B, F, T)}, got {tuple(lambda_enh.shape)}")
+    lambda_enh = _arg(lambda_enh, stft.device, torch.complex64, (B, F, T), "lambda_enh")
     out = torch.empty_like(stft)
     inv = torch.empty((B, T, F), dtype=torch.float32, device=stft.device) if want_inv_lambda else None
     status = torch.zeros((B,), dtype=torch.int32, device=stft.device)
-    with _ctx(stft.device):
-        _lib.check(_lib.library().setk_wpe_step(
-            _lib.ptr(stft), _lib.ptr(lambda_enh), B, C, F, T, int(taps), int(delay), int(context),
-            _lib.ptr(out), _lib.ptr(inv), _lib.ptr(status), _lib.current_stream(stft.device)))
+    _launch(stft.device, "setk_wpe_step", _lib.ptr(stft), _lib.ptr(lambda_enh), B, C, F, T, int(taps), int(delay),
+            int(context), _lib.ptr(out), _lib.ptr(inv), _lib.ptr(status))
     return out, inv, status
 
 
 def covariance(stft, mask, clip_mask=False, mask_ft=False):
-    """compute_covar batched: stft (B,C,F,T) c64, mask (B,T,F) -> (B,F,C,C) c64."""
-    stft = stft.contiguous()
-    if stft.dtype != torch.complex64:
-        stft = stft.to(torch.complex64)
+    """compute_covar batched: stft (B,C,F,T) c64, mask (B,T,F) (or (B,F,T) with mask_ft) -> (B,F,C,C) c64."""
+    stft = _arg(stft, None, torch.complex64, (None,) * 4, "stft")
     B, C, F, T = stft.shape
-    mask = _f32(mask, stft.device)
+    mask = _arg(mask, stft.device, torch.float32, (B, F, T) if mask_ft else (B, T, F), "mask")
     R = torch.empty((B, F, C, C), dtype=torch.complex64, device=stft.device)
     flags = (_lib.F_CLIP_MASK if clip_mask else 0) | (_lib.F_MASK_FT if mask_ft else 0)
-    with _ctx(stft.device):
-        _lib.check(_lib.library().setk_cov(_lib.ptr(stft), _lib.ptr(mask), flags, B, C, F, T,
-                                           _lib.ptr(R), _lib.current_stream(stft.device)))
+    _launch(stft.device, "setk_cov", _lib.ptr(stft), _lib.ptr(mask), flags, B, C, F, T, _lib.ptr(R))
     return R
+
+
+def _square(Rs):
+    """Rs through _arg as a (B,F,C,C) stack of square matrices, dtype kept."""
+    Rs = _arg(Rs, None, None, (None,) * 4, "Rs")
+    if Rs.shape[3] != Rs.shape[2]:
+        raise ValueError(f"Rs must be (B, F, C, C), got {tuple(Rs.shape)}")
+    return Rs
 
 
 def weights(kind, Rs, Rn=None, Ry=None, beta=0.0, ref_channel=-1, rank1=_lib.RANK1_NONE,
@@ -353,84 +319,70 @@ def weights(kind, Rs, Rn=None, Ry=None, beta=0.0, ref_channel=-1, rank1=_lib.RAN
     Per-bin weight solve.  Rs/Rn/Ry (B,F,C,C) complex64|complex128 (same dtype).
     Returns (w (B,F,C), status (B,) int32 tensor, ref_used (B,) int32 tensor).
     """
-    Rs = Rs.contiguous()
+    Rs = _square(Rs)
     B, F, C, _ = Rs.shape
     dt = _dtype_code(Rs)
-    for m in (Rn, Ry):
-        if m is not None and (m.dtype != Rs.dtype or m.shape != Rs.shape):
-            raise ValueError("Rs / Rn / Ry must share dtype and shape")
-    Rn = None if Rn is None else Rn.contiguous()
-    Ry = None if Ry is None else Ry.contiguous()
+    Rn, Ry = (_arg(m, Rs.device, None, (B, F, C, C), what) for m, what in ((Rn, "Rn"), (Ry, "Ry")))
+    if any(m is not None and m.dtype != Rs.dtype for m in (Rn, Ry)):
+        raise ValueError("Rs / Rn / Ry must share dtype and shape")
     out_dtype = Rs.dtype if out_dtype is None else out_dtype
     w = torch.empty((B, F, C), dtype=out_dtype, device=Rs.device)
     status = torch.zeros((B,), dtype=torch.int32, device=Rs.device)
     ref_used = torch.full((B,), -1, dtype=torch.int32, device=Rs.device)
-    with _ctx(Rs.device):
-        _lib.check(_lib.library().setk_weights(
-            int(kind), float(beta), int(ref_channel), int(rank1), int(bool(ban)), _lib.ptr(Rs),
-            _lib.ptr(Rn), _lib.ptr(Ry), dt, B, F, C, _lib.ptr(w), _dtype_code(w), _lib.ptr(status),
-            _lib.ptr(ref_used), _lib.current_stream(Rs.device)))
+    _launch(Rs.device, "setk_weights", int(kind), float(beta), int(ref_channel), int(rank1), int(bool(ban)),
+            _lib.ptr(Rs), _lib.ptr(Rn), _lib.ptr(Ry), dt, B, F, C, _lib.ptr(w), _dtype_code(w), _lib.ptr(status),
+            _lib.ptr(ref_used))
     return w, status, ref_used
 
 
 def ban(weight, Rn):
-    """do_ban batched: weight (B,F,C), Rn (B,F,C,C), same complex dtype."""
-    Rn = Rn.contiguous()
-    weight = weight.to(Rn.dtype).contiguous()
+    """do_ban batched: weight (B,F,C), Rn (B,F,C,C); weight is taken in Rn's complex dtype."""
+    weight = _arg(weight, None, None, (None,) * 3, "weight")
     B, F, C = weight.shape
+    Rn = _arg(Rn, weight.device, None, (B, F, C, C), "Rn")
+    weight = weight.to(Rn.dtype)
     out = torch.empty_like(weight)
-    with _ctx(Rn.device):
-        _lib.check(_lib.library().setk_ban(_lib.ptr(weight), _lib.ptr(Rn), _dtype_code(Rn), B, F, C,
-                                           _lib.ptr(out), _lib.current_stream(Rn.device)))
+    _launch(weight.device, "setk_ban", _lib.ptr(weight), _lib.ptr(Rn), _dtype_code(Rn), B, F, C, _lib.ptr(out))
     return out
 
 
 def rank1(Rs, Rn=None):
     """rank1_constraint batched.  Returns (R1 (B,F,C,C), status (B,))."""
-    Rs = Rs.contiguous()
+    Rs = _square(Rs)
     B, F, C, _ = Rs.shape
-    Rn = None if Rn is None else Rn.to(Rs.dtype).contiguous()
+    Rn = _arg(Rn, Rs.device, Rs.dtype, (B, F, C, C), "Rn")
     out = torch.empty_like(Rs)
     status = torch.zeros((B,), dtype=torch.int32, device=Rs.device)
-    with _ctx(Rs.device):
-        _lib.check(_lib.library().setk_rank1(_lib.ptr(Rs), _lib.ptr(Rn), _dtype_code(Rs), B, F, C,
-                                             _lib.ptr(out), _lib.ptr(status),
-                                             _lib.current_stream(Rs.device)))
+    _launch(Rs.device, "setk_rank1", _lib.ptr(Rs), _lib.ptr(Rn), _dtype_code(Rs), B, F, C, _lib.ptr(out),
+            _lib.ptr(status))
     return out, status
 
 
 def apply_weights(stft, weight, post_mask=None):
-    """Beamformer.beamform batched: (B,C,F,T) x (B,F,C) -> (B,F,T) complex64."""
-    stft = stft.contiguous()
-    if stft.dtype != torch.complex64:
-        stft = stft.to(torch.complex64)
+    """Beamformer.beamform batched: (B,C,F,T) x (B,F,C) [x post_mask (B,T,F)] -> (B,F,T) complex64."""
+    stft = _arg(stft, None, torch.complex64, (None,) * 4, "stft")
     B, C, F, T = stft.shape
-    weight = weight.contiguous()
-    if post_mask is not None:
-        post_mask = _f32(post_mask, stft.device)
+    weight = _arg(weight, stft.device, None, (B, F, C), "weight")
+    post_mask = _arg(post_mask, stft.device, torch.float32, (B, T, F), "post_mask")
     enh = torch.empty((B, F, T), dtype=torch.complex64, device=stft.device)
-    with _ctx(stft.device):
-        _lib.check(_lib.library().setk_apply(_lib.ptr(stft), _lib.ptr(weight), _dtype_code(weight),
-                                             _lib.ptr(post_mask), B, C, F, T, _lib.ptr(enh),
-                                             _lib.current_stream(stft.device)))
+    _launch(stft.device, "setk_apply", _lib.ptr(stft), _lib.ptr(weight), _dtype_code(weight), _lib.ptr(post_mask),
+            B, C, F, T, _lib.ptr(enh))
     return enh
 
 
 def float_to_pcm16(wave):
-    wave = wave.contiguous()
+    wave = _arg(wave, None, torch.float32, None, "wave")
     pcm = torch.empty(wave.shape, dtype=torch.int16, device=wave.device)
-    with _ctx(wave.device):
-        _lib.check(_lib.library().setk_float_to_pcm16(_lib.ptr(wave), wave.numel(), _lib.ptr(pcm),
-                                                      _lib.current_stream(wave.device)))
+    _launch(wave.device, "setk_float_to_pcm16", _lib.ptr(wave), wave.numel(), _lib.ptr(pcm))
     return pcm
 
 
 def pcm16_to_float(pcm):
-    pcm = pcm.contiguous()
+    pcm = _arg(pcm, None, None, None, "pcm")
+    if pcm.dtype != torch.int16:
+        raise ValueError(f"pcm16_to_float: pcm must be int16, got {pcm.dtype}")
     wave = torch.empty(pcm.shape, dtype=torch.float32, device=pcm.device)
-    with _ctx(pcm.device):
-        _lib.check(_lib.library().setk_pcm16_to_float(_lib.ptr(pcm), pcm.numel(), _lib.ptr(wave),
-                                                      _lib.current_stream(pcm.device)))
+    _launch(pcm.device, "setk_pcm16_to_float", _lib.ptr(pcm), pcm.numel(), _lib.ptr(wave))
     return wave
 
 
@@ -440,43 +392,35 @@ def cm_masks(blobs, T, F, out=None):
     blobs: uint8 [B][slot_bytes] device tensor, one matrix per slot as it lies in the archive behind
     the "CM " token (slot_bytes a multiple of 16).  Returns (masks, status int32 [B]).
     """
+    blobs = _arg(blobs, None, None, None, "blobs")
     if blobs.dtype != torch.uint8 or blobs.dim() != 2:
         raise ValueError("cm_masks: blobs must be uint8 [B][slot_bytes]")
-    blobs = blobs.contiguous()
     B = blobs.shape[0]
     if out is None:
         out = torch.empty((B, T, F), dtype=torch.float32, device=blobs.device)
+    else:
+        out = _out(out, blobs.device, torch.float32, (B, T, F), "cm_masks: out")
     status = torch.zeros((B,), dtype=torch.int32, device=blobs.device)
-    with _ctx(blobs.device):
-        _lib.check(_lib.library().setk_cm_masks(_lib.ptr(blobs), blobs.shape[1], B, T, F, _lib.ptr(out),
-                                                _lib.ptr(status), _lib.current_stream(blobs.device)))
+    _launch(blobs.device, "setk_cm_masks", _lib.ptr(blobs), blobs.shape[1], B, T, F, _lib.ptr(out), _lib.ptr(status))
     return out, status
 
 
 # ---------------------------------------------------------------------------
 # spatial features on explicit STFTs (libs/spatial.py of the reference; csrc/spatial.cu)
 # ---------------------------------------------------------------------------
-def _c64(t, device=None):
-    t = torch.as_tensor(t) if device is None else torch.as_tensor(t, device=device)
-    if t.dtype != torch.complex64:
-        t = t.to(torch.complex64)
-    return t.contiguous()
-
-
 def ipd(si, sj, mode=0):
     """spatial.ipd: si, sj (..., T, F) complex64 -> float32 (..., T, F) (mode 0/1) or (..., T, 2F)."""
-    si, sj = _c64(si), _c64(sj, si.device if torch.is_tensor(si) else None)
-    if si.shape != sj.shape or si.dim() < 2:
-        raise ValueError(f"ipd: shapes {tuple(si.shape)} / {tuple(sj.shape)}")
+    si = _arg(si, None, torch.complex64, None, "ipd: si")
+    if si.dim() < 2:
+        raise ValueError(f"ipd: si must be (..., T, F), got {tuple(si.shape)}")
+    sj = _arg(sj, si.device, torch.complex64, si.shape, "ipd: sj")
     F = si.shape[-1]
     rows = si.numel() // F
     shape = list(si.shape)
     if mode == 2:
         shape[-1] = 2 * F
     out = torch.empty(shape, dtype=torch.float32, device=si.device)
-    with _ctx(si.device):
-        _lib.check(_lib.library().setk_ipd(_lib.ptr(si), _lib.ptr(sj), rows, F, int(mode),
-                                           _lib.ptr(out), _lib.current_stream(si.device)))
+    _launch(si.device, "setk_ipd", _lib.ptr(si), _lib.ptr(sj), rows, F, int(mode), _lib.ptr(out))
     return out
 
 
@@ -485,25 +429,20 @@ def directional_feats(stft, steer, pairs=None):
     spatial.directional_feats batched: stft (B,M,F,T) complex64, steer (M,F) or (B,M,F)
     complex -> (B,T,F) float64.  pairs: list of (i, j) or None (all i < j).
     """
-    stft = _c64(stft)
-    if stft.dim() != 4:
-        raise ValueError(f"stft must be (B, M, F, T), got {tuple(stft.shape)}")
+    stft = _arg(stft, None, torch.complex64, (None,) * 4, "stft")
     B, M, F, T = stft.shape
-    steer = torch.as_tensor(steer, device=stft.device).to(torch.complex128).contiguous()
-    batched = steer.dim() == 3
-    if tuple(steer.shape[-2:]) != (M, F) or (batched and steer.shape[0] != B):
-        raise ValueError(f"steer vector must be ({M}, {F}) or ({B}, {M}, {F}), got {tuple(steer.shape)}")
-    p_t, n_pairs = None, 0
-    if pairs is not None:
-        p_t = torch.as_tensor(pairs, dtype=torch.int32, device=stft.device).reshape(-1, 2).contiguous()
+    batched = np.ndim(steer) == 3
+    steer = _arg(steer, stft.device, torch.complex128, (B, M, F) if batched else (M, F), "steer vector")
+    p_t = _arg(pairs, stft.device, torch.int32, None, "df_pair")
+    n_pairs = 0
+    if p_t is not None:
+        p_t = p_t.reshape(-1, 2)
         n_pairs = p_t.shape[0]
         if n_pairs == 0 or int(p_t.min()) < 0 or int(p_t.max()) >= M:
             raise ValueError(f"df_pair entries must lie in [0, {M})")
     out = torch.empty((B, T, F), dtype=torch.float64, device=stft.device)
-    with _ctx(stft.device):
-        _lib.check(_lib.library().setk_directional_feats(
-            _lib.ptr(stft), _lib.ptr(steer), int(batched), _lib.ptr(p_t), n_pairs, B, M, F, T,
-            _lib.ptr(out), _lib.current_stream(stft.device)))
+    _launch(stft.device, "setk_directional_feats", _lib.ptr(stft), _lib.ptr(steer), int(batched), _lib.ptr(p_t),
+            n_pairs, B, M, F, T, _lib.ptr(out))
     return out
 
 
@@ -513,41 +452,32 @@ def gcc_phat(si, sj, omega, tau, normalize=True, apply_floor=True, out=None):
     and tau (D,) float64 -> (T,D) float64.  With `out` given the pair is ADDED to it
     (srp_phat_linear).
     """
-    si = _c64(si)
-    sj = _c64(sj, si.device)
-    if si.dim() != 2 or si.shape != sj.shape:
-        raise ValueError(f"gcc_phat: si/sj must be (T, F), got {tuple(si.shape)} / {tuple(sj.shape)}")
+    si = _arg(si, None, torch.complex64, (None, None), "gcc_phat: si")
     T, F = si.shape
-    omega = torch.as_tensor(omega, dtype=torch.float64, device=si.device).contiguous()
-    tau = torch.as_tensor(tau, dtype=torch.float64, device=si.device).contiguous()
-    if omega.numel() != F:
-        raise ValueError(f"gcc_phat: {omega.numel()} frequencies for {F} bins")
-    D = tau.numel()
-    lib = _lib.library()
-    work = torch.empty((int(lib.setk_gcc_phat_work_doubles(T, F, D)),), dtype=torch.float64,
-                       device=si.device)
+    dev = si.device
+    sj = _arg(sj, dev, torch.complex64, (T, F), "gcc_phat: sj")
+    omega = _arg(omega, dev, torch.float64, (F,), "gcc_phat: omega")
+    tau = _arg(tau, dev, torch.float64, (None,), "gcc_phat: tau")
+    D = tau.shape[0]
+    work = torch.empty((int(_lib.library().setk_gcc_phat_work_doubles(T, F, D)),), dtype=torch.float64, device=dev)
     accumulate = out is not None
-    if out is None:
-        out = torch.empty((T, D), dtype=torch.float64, device=si.device)
-    with _ctx(si.device):
-        _lib.check(lib.setk_gcc_phat(_lib.ptr(si), _lib.ptr(sj), T, F, _lib.ptr(omega), _lib.ptr(tau), D,
-                                     int(bool(normalize)), int(bool(apply_floor)), int(accumulate),
-                                     _lib.ptr(work), _lib.ptr(out), _lib.current_stream(si.device)))
+    if accumulate:
+        out = _out(out, dev, torch.float64, (T, D), "gcc_phat: out")
+    else:
+        out = torch.empty((T, D), dtype=torch.float64, device=dev)
+    _launch(dev, "setk_gcc_phat", _lib.ptr(si), _lib.ptr(sj), T, F, _lib.ptr(omega), _lib.ptr(tau), D,
+            int(bool(normalize)), int(bool(apply_floor)), int(accumulate), _lib.ptr(work), _lib.ptr(out))
     return out
 
 
 def msc(spec, context=1, normalize=True):
     """spatial.msc: spec (N,T,F) complex64 -> (T,F) float64."""
-    spec = _c64(spec)
-    if spec.dim() != 3:
-        raise ValueError(f"msc: spectrogram must be (N, T, F), got {tuple(spec.shape)}")
+    spec = _arg(spec, None, torch.complex64, (None,) * 3, "msc: spectrogram")
     N, T, F = spec.shape
-    lib = _lib.library()
-    work = torch.empty((int(lib.setk_msc_work_doubles(T, F)),), dtype=torch.float64, device=spec.device)
+    work = torch.empty((int(_lib.library().setk_msc_work_doubles(T, F)),), dtype=torch.float64, device=spec.device)
     out = torch.empty((T, F), dtype=torch.float64, device=spec.device)
-    with _ctx(spec.device):
-        _lib.check(lib.setk_msc(_lib.ptr(spec), N, T, F, int(context), int(bool(normalize)),
-                                _lib.ptr(work), _lib.ptr(out), _lib.current_stream(spec.device)))
+    _launch(spec.device, "setk_msc", _lib.ptr(spec), N, T, F, int(context), int(bool(normalize)), _lib.ptr(work),
+            _lib.ptr(out))
     return out
 
 
@@ -567,37 +497,21 @@ def ssl(stft, steer, backend="ml", mask=None, windows=None, pairs=None, compress
     """
     if backend not in _SSL_BACKENDS:
         raise ValueError(f"unknown SSL backend {backend!r}")
-    stft = _c64(stft)
-    if stft.dim() != 4:
-        raise ValueError(f"stft must be (B, M, F, T), got {tuple(stft.shape)}")
+    stft = _arg(stft, None, torch.complex64, (None,) * 4, "stft")
     B, M, F, T = stft.shape
     dev = stft.device
-    steer = torch.as_tensor(steer, device=dev).to(torch.complex128).contiguous()
-    if steer.dim() != 3 or steer.shape[1] != M:
-        raise ValueError(f"steer vector must be (A, {M}, F), got {tuple(steer.shape)}")
+    steer = _arg(steer, dev, torch.complex128, (None, M, None), "steer vector")   # its bins: setk_ssl checks
     A = steer.shape[0]
-    N = 1
-    if mask is not None:
-        mask = _f32(mask, dev)
-        if mask.dim() != 4 or mask.shape[0] != B or tuple(mask.shape[2:]) != (T, F):
-            raise ValueError(f"mask must be ({B}, N, {T}, {F}), got {tuple(mask.shape)}")
-        N = mask.shape[1]
-    win = np.array([[[0, T]]] * B if windows is None else windows, dtype=np.int32).reshape(B, -1, 2)
-    win = np.ascontiguousarray(win)
-    W = win.shape[1]
-    pr = None
-    P = 0
-    if pairs is not None:
-        pr = np.ascontiguousarray(np.array(pairs, dtype=np.int32).reshape(-1, 2))
-        P = pr.shape[0]
+    mask = _arg(mask, dev, torch.float32, (B, None, T, F), "mask")
+    N = 1 if mask is None else mask.shape[1]
+    win, win_p = _host_i32(np.reshape([[0, T]] * B if windows is None else windows, (B, -1, 2)))
+    pr, pr_p = _host_i32(None if pairs is None else np.reshape(pairs, (-1, 2)))
+    W, P = win.shape[1], 0 if pr is None else pr.shape[0]
     scores = torch.empty((B, N, W, A), dtype=torch.float64, device=dev)
     index = torch.empty((B, N, W), dtype=torch.int32, device=dev)
-    with _ctx(dev):
-        _lib.check(_lib.library().setk_ssl(
-            _SSL_BACKENDS[backend], _lib.ptr(stft), B, M, F, T, _lib.ptr(steer), A, steer.shape[2],
-            _lib.ptr(mask), N, ctypes.c_void_p(win.ctypes.data), W,
-            None if pr is None else ctypes.c_void_p(pr.ctypes.data), P, float(compression), float(eps),
-            int(bool(normalize)), _lib.ptr(scores), _lib.ptr(index), _lib.current_stream(dev)))
+    _launch(dev, "setk_ssl", _SSL_BACKENDS[backend], _lib.ptr(stft), B, M, F, T, _lib.ptr(steer), A, steer.shape[2],
+            _lib.ptr(mask), N, win_p, W, pr_p, P, float(compression), float(eps), int(bool(normalize)),
+            _lib.ptr(scores), _lib.ptr(index))
     return scores, index
 
 
@@ -609,16 +523,12 @@ def auxiva_from_stft(stft, num_epochs=20):
     auxiva(X, epochs) batched (apply_auxiva.py:24-57).
     stft (B,N,F,T) complex64 -> (separated sources (B,N,F,T) complex128, status (B,) int32).
     """
-    stft = _c64(stft)
-    if stft.dim() != 4:
-        raise ValueError(f"stft must be (B, N, F, T), got {tuple(stft.shape)}")
+    stft = _arg(stft, None, torch.complex64, (None,) * 4, "stft")
     B, N, F, T = stft.shape
     out = torch.empty((B, N, F, T), dtype=torch.complex128, device=stft.device)
     status = torch.zeros((B,), dtype=torch.int32, device=stft.device)
-    with _ctx(stft.device):
-        _lib.check(_lib.library().setk_auxiva_stft(
-            _lib.ptr(stft), B, N, F, T, int(num_epochs), _lib.ptr(out), _lib.ptr(status),
-            _lib.current_stream(stft.device)))
+    _launch(stft.device, "setk_auxiva_stft", _lib.ptr(stft), B, N, F, T, int(num_epochs), _lib.ptr(out),
+            _lib.ptr(status))
     return out, status
 
 
@@ -656,24 +566,16 @@ def ns_from_stft(stft, n_frames=None, config=None, gain=True, enh=True, eps=1e-7
     stft (B,F,T) complex64; n_frames (B,) int or None (every utterance has T frames).
     Returns (gain (B,T,F) float64 or None, enh (B,F,T) complex64 or None).
     """
-    stft = _c64(stft)
-    if stft.dim() != 3:
-        raise ValueError(f"stft must be (B, F, T), got {tuple(stft.shape)}")
+    stft = _arg(stft, None, torch.complex64, (None,) * 3, "stft")
     if not (gain or enh):
         raise ValueError("ns_from_stft: ask for the gain, the enhanced STFT or both")
     B, F, T = stft.shape
     dev = stft.device
-    nf = None
-    if n_frames is not None:
-        nf = torch.as_tensor(n_frames, device=dev).to(torch.int32).contiguous()
-        if nf.shape != (B,):
-            raise ValueError(f"n_frames must have shape ({B},)")
+    nf = _arg(n_frames, dev, torch.int32, (B,), "n_frames")
     g = torch.empty((B, T, F), dtype=torch.float64, device=dev) if gain else None
     e = torch.empty((B, F, T), dtype=torch.complex64, device=dev) if enh else None
     cfg, window = imcra_config(config, eps)
-    with _ctx(dev):
-        _lib.check(_lib.library().setk_ns_imcra(ctypes.byref(cfg), _lib.ptr(stft), _lib.ptr(nf), B, F, T,
-                                                _lib.ptr(g), _lib.ptr(e), _lib.current_stream(dev)))
+    _launch(dev, "setk_ns_imcra", ctypes.byref(cfg), _lib.ptr(stft), _lib.ptr(nf), B, F, T, _lib.ptr(g), _lib.ptr(e))
     del window
     return g, e
 
@@ -720,18 +622,15 @@ def rir_image(room, beta, source, receivers, n_samples, sr=16000, c=340, order=-
                       "cuda" if torch.cuda.is_available() else "cpu")
     dev = torch.device(device)
 
-    def f64(t, shape):
-        t = torch.as_tensor(t, dtype=torch.float64, device=dev).contiguous()
-        return t.reshape(shape) if t.dim() == len(shape) - 1 else t
+    def f64(t, shape, what):      # one problem (B = 1) may drop the leading B
+        single = np.ndim(t) == len(shape) - 1 and shape[0] in (None, 1)
+        t = _arg(t, dev, torch.float64, shape[1:] if single else shape, what)
+        return t[None] if single else t
 
-    room = f64(room, (1, 3))
+    room = f64(room, (None, 3), "room")
     B = room.shape[0]
-    beta, source, receivers = f64(beta, (1, 6)), f64(source, (1, 3)), f64(receivers, (1, -1, 3))
-    if room.shape != (B, 3) or beta.shape != (B, 6) or source.shape != (B, 3) or receivers.dim() != 3 \
-            or receivers.shape[0] != B or receivers.shape[2] != 3:
-        raise ValueError(f"shapes room {tuple(room.shape)}, beta {tuple(beta.shape)}, source "
-                         f"{tuple(source.shape)}, receivers {tuple(receivers.shape)}: want (B,3), (B,6), "
-                         "(B,3), (B,M,3)")
+    beta, source = f64(beta, (B, 6), "beta"), f64(source, (B, 3), "source")
+    receivers = f64(receivers, (B, None, 3), "receivers")
     M, L = receivers.shape[1], int(n_samples)
     out = torch.empty((B, M, max(L, 0)), dtype=torch.float32, device=dev)
     status = torch.zeros(B, dtype=torch.int32, device=dev)
@@ -739,10 +638,8 @@ def rir_image(room, beta, source, receivers, n_samples, sr=16000, c=340, order=-
     cfg = _lib.RirConfig(sound_velocity=float(c), samp_frequency=float(sr), azimuth=az, elevation=el,
                          n_samples=L, order=int(order), mic_type=_lib.MIC_TYPES.index(mic_type),
                          hp_filter=int(bool(hp_filter)))
-    with _ctx(dev):
-        _lib.check(_lib.library().setk_rir_image(ctypes.byref(cfg), _lib.ptr(room), _lib.ptr(beta),
-                                                 _lib.ptr(source), _lib.ptr(receivers), B, M, _lib.ptr(out),
-                                                 _lib.ptr(status), _lib.current_stream(dev)))
+    _launch(dev, "setk_rir_image", ctypes.byref(cfg), _lib.ptr(room), _lib.ptr(beta), _lib.ptr(source),
+            _lib.ptr(receivers), B, M, _lib.ptr(out), _lib.ptr(status))
     bad = torch.nonzero(status).flatten().tolist()
     if bad:
         raise ValueError(f"rir_image: the response of problem {bad[0]} is not finite or out of range "
@@ -753,15 +650,6 @@ def rir_image(room, beta, source, receivers, n_samples, sr=16000, c=340, order=-
 # ---------------------------------------------------------------------------
 # Speech + RIR + noise mixtures (wav_simulate.py of the reference; csrc/simu.cu, setk_b200/simu.py)
 # ---------------------------------------------------------------------------
-def _lens(v, B, what):
-    if v is None:
-        return None
-    a = np.ascontiguousarray(np.broadcast_to(np.asarray(v, dtype=np.int32), (B,)))
-    if a.shape != (B,):
-        raise ValueError(f"{what} must be one length or ({B},)")
-    return a
-
-
 def convolve(x, h, n_out=None, s_len=None, h_len=None, out=None):
     """
     ss.convolve(x[None], h)[..., :n_out] of add_room_response (wav_simulate.py:29-54, without the
@@ -776,30 +664,22 @@ def convolve(x, h, n_out=None, s_len=None, h_len=None, out=None):
     if single:
         x = x[None]
         h = h.reshape(1, 1, -1) if h.dim() == 1 else h[None]
-    if x.dim() != 2 or h.dim() != 3 or h.shape[0] != x.shape[0]:
-        raise ValueError(f"convolve: x {tuple(x.shape)} and h {tuple(h.shape)}: want (B,S) and (B,M,L)")
     dev = h.device if h.device.type != "cpu" else x.device
-    x = _f32(x, dev).contiguous()
-    h = _f32(h, dev).contiguous()
+    x = _arg(x, dev, torch.float32, (None, None), "convolve: x")
     B, Sx = x.shape
+    h = _arg(h, dev, torch.float32, (B, None, None), "convolve: h")
     M, Lh = h.shape[1], h.shape[2]
-    s_l, h_l = _lens(s_len, B, "s_len"), _lens(h_len, B, "h_len")
+    _, s_p = _host_i32(s_len, (B,))
+    _, h_p = _host_i32(h_len, (B,))
     if n_out is None:
-        n_l = s_l if s_l is not None else np.full(B, Sx, np.int32)
-    else:
-        n_l = _lens(n_out, B, "n_out")
+        n_out = Sx if s_len is None else s_len
+    n_l, n_p = _host_i32(n_out, (B,))
     Ny = int(n_l.max()) if B else 0
     if out is None:
         out = torch.empty((B, M, max(Ny, 0)), dtype=torch.float32, device=dev)
-    elif out.shape != (B, M, Ny) or out.dtype != torch.float32 or not out.is_contiguous():
-        raise ValueError(f"convolve: out must be a contiguous float32 ({B}, {M}, {Ny}) tensor")
-
-    def p(a):
-        return None if a is None else a.ctypes.data_as(ctypes.POINTER(ctypes.c_int32))
-
-    with _ctx(dev):
-        _lib.check(_lib.library().setk_convolve(_lib.ptr(x), Sx, _lib.ptr(h), Lh, B, M, p(s_l), p(h_l), p(n_l),
-                                                _lib.ptr(out), Ny, _lib.current_stream(dev)))
+    else:
+        out = _out(out, dev, torch.float32, (B, M, Ny), "convolve: out")
+    _launch(dev, "setk_convolve", _lib.ptr(x), Sx, _lib.ptr(h), Lh, B, M, s_p, h_p, n_p, _lib.ptr(out), Ny)
     return out[0] if single else out
 
 
@@ -812,6 +692,8 @@ def simulate_mix(pool, mixes, terms, n_channels, n_speakers, n_samples, pcm16=Fa
     shape M, K, n_pitch.  Returns (mix (B,M,n_pitch), spk (B,K,n_pitch) or None, noise (B,n_pitch) or
     None, factor (B,) float64), float32 or, with pcm16, int16 as write_wav stores them.
     """
+    # the pool holds every image of the batch: it is refused rather than converted, since a silent
+    # float32 copy would double the largest buffer of the call
     pool = pool.reshape(-1)
     if pool.dtype != torch.float32 or not pool.is_contiguous():
         raise ValueError("simulate_mix: pool must be a contiguous float32 tensor")
@@ -825,11 +707,9 @@ def simulate_mix(pool, mixes, terms, n_channels, n_speakers, n_samples, pcm16=Fa
     s = torch.empty((B, K, max(N, 0)), dtype=dt, device=dev) if spk else None
     nz = torch.empty((B, max(N, 0)), dtype=dt, device=dev) if noise else None
     factor = torch.empty((B,), dtype=torch.float64, device=dev)
-    with _ctx(dev):
-        _lib.check(_lib.library().setk_simulate_mix(
-            _lib.ptr(pool), pool.numel(), ctypes.cast(mx, ctypes.c_void_p), B, ctypes.cast(tm, ctypes.c_void_p), T,
-            M, K, N, int(bool(pcm16)), _lib.ptr(mix), _lib.ptr(s), _lib.ptr(nz), _lib.ptr(factor),
-            _lib.current_stream(dev)))
+    _launch(dev, "setk_simulate_mix", _lib.ptr(pool), pool.numel(), ctypes.cast(mx, ctypes.c_void_p), B,
+            ctypes.cast(tm, ctypes.c_void_p), T, M, K, N, int(bool(pcm16)), _lib.ptr(mix), _lib.ptr(s), _lib.ptr(nz),
+            _lib.ptr(factor))
     return mix, s, nz, factor
 
 
@@ -841,21 +721,16 @@ SEP_SCRATCH_BYTES = 4 << 30   # bss_eval splits a batch so that one call's scrat
 
 def _sep_inputs(est, ref, n_samples, who):
     est, ref = torch.as_tensor(est), torch.as_tensor(ref)
-    if est.dim() != 3 or est.shape != ref.shape:
-        raise ValueError(f"{who}: est {tuple(est.shape)} and ref {tuple(ref.shape)} must both be (B, N, S)")
     dev = ref.device if ref.device.type != "cpu" else est.device
-    est, ref = _f32(est, dev), _f32(ref, dev)
+    est = _arg(est, dev, torch.float32, (None,) * 3, f"{who}: est")
+    ref = _arg(ref, dev, torch.float32, est.shape, f"{who}: ref")
     B, N, S = est.shape
     lens = None
     if n_samples is not None:
-        lens = np.ascontiguousarray(np.broadcast_to(np.asarray(n_samples, dtype=np.int64), (B,))).astype(np.int32)
+        lens = np.broadcast_to(np.asarray(n_samples, dtype=np.int64), (B,))   # checked before the int32 cast
         if lens.size and (lens.min() < 1 or lens.max() > S):
             raise ValueError(f"{who}: n_samples must lie in [1, {S}]")
     return est, ref, lens, dev
-
-
-def _i32p(a):
-    return None if a is None else a.ctypes.data_as(ctypes.POINTER(ctypes.c_int32))
 
 
 def bss_eval_batch_step(B, N, S, flen=512):
@@ -886,13 +761,11 @@ def bss_eval(est, ref, n_samples=None, flen=512):
     dropped = torch.zeros((B,), dtype=torch.int32, device=dev)
     status = torch.zeros((B,), dtype=torch.int32, device=dev)
     step = bss_eval_batch_step(B, N, S, L)
-    with _ctx(dev):
-        for b0 in range(0, B, step):
-            b1 = min(B, b0 + step)
-            _lib.check(_lib.library().setk_bss_eval(
-                _lib.ptr(est[b0:b1]), _lib.ptr(ref[b0:b1]), _i32p(None if lens is None else lens[b0:b1]),
-                b1 - b0, N, S, L, _lib.ptr(crit[b0:b1]), _lib.ptr(dropped[b0:b1]), _lib.ptr(status[b0:b1]),
-                _lib.current_stream(dev)))
+    for b0 in range(0, B, step):
+        b1 = min(B, b0 + step)
+        _, lens_p = _host_i32(None if lens is None else lens[b0:b1])
+        _launch(dev, "setk_bss_eval", _lib.ptr(est[b0:b1]), _lib.ptr(ref[b0:b1]), lens_p, b1 - b0, N, S, L,
+                _lib.ptr(crit[b0:b1]), _lib.ptr(dropped[b0:b1]), _lib.ptr(status[b0:b1]))
     return crit, dropped, status
 
 
@@ -904,8 +777,6 @@ def si_snr(est, ref, n_samples=None, remove_dc=True, eps=1e-8):
     est, ref, lens, dev = _sep_inputs(est, ref, n_samples, "si_snr")
     B, N, S = est.shape
     out = torch.empty((B, N, N), dtype=torch.float64, device=dev)
-    with _ctx(dev):
-        _lib.check(_lib.library().setk_si_snr(_lib.ptr(est), _lib.ptr(ref), _i32p(lens), B, N, S,
-                                              int(bool(remove_dc)), float(eps), _lib.ptr(out),
-                                              _lib.current_stream(dev)))
+    _launch(dev, "setk_si_snr", _lib.ptr(est), _lib.ptr(ref), _host_i32(lens)[1], B, N, S, int(bool(remove_dc)),
+            float(eps), _lib.ptr(out))
     return out
