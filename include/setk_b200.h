@@ -265,6 +265,60 @@ int setk_cgmm_stft(const void* stft, int32_t B, int32_t C, int32_t F, int32_t T,
                    int32_t num_iters, const float* init_gamma, int32_t update_alpha, float* masks,
                    uint32_t* status, void* stream);
 
+#define SETK_PERMU_MAX_ROWS 64   /* rows of a permutation-alignment sub-band plan */
+
+/*
+ * CACGMM speaker-mask estimation from audio: the tile STFT, then
+ * CacgmmTrainer(stft, num_classes, gamma=init, cgmm_init=..., update_alpha=...).train(num_iters)
+ * (scripts/sptk/libs/cluster.py:468-535 with 39-45, 94-136, 290-393) for every utterance of the
+ * batch, then, when permu_plan is given, permu_aligner (cluster.py:48-91) on the fp64 posteriors,
+ * and the CLI's transpose (scripts/sptk/estimate_cacgmm_masks.py:40-63).  fp64 arithmetic after
+ * the complex64 STFT, on the observations normalised over channels.
+ *
+ *   num_classes  2..4
+ *   init_gamma   f64 [B][K][T][F] starting posteriors (the reference's numpy draw, or a given
+ *                mask), or NULL with cgmm_init && num_classes == 2
+ *   cgmm_init    nonzero with num_classes == 2: the start B_0 = sum_t z z^H / T, B_1 = I and one
+ *                E-step (cluster.py:495-506); otherwise the start is init_gamma, no E-step
+ *   update_alpha nonzero: the priors follow mean_t gamma (cluster.py:364-365)
+ *   permu_plan   host i32 [R][3] rows (iterations, first bin, end bin), 0 <= lo < hi <= F,
+ *                R <= SETK_PERMU_MAX_ROWS, or NULL / R = 0: no alignment
+ *   masks        f32 [B][K][T][F], 0 past each utterance's frames
+ *   status       u32 [B] or NULL, OR-ed SETK_ST_NO_CONVERGE (caller zeroes it)
+ * num_iters = 0 returns the start.  SETK_EINVAL for a null buffer, K outside 2..4, C < 2,
+ * num_iters < 0, a NULL start without cgmm_init && K == 2, or a bad plan row; SETK_EUNSUPPORTED
+ * unless n_fft is 512 or 1024 (the tile STFT).
+ */
+int setk_cacgmm_masks(setk_plan_t* plan, const float* audio, const int32_t* n_samples, int32_t B, int32_t N,
+                      int32_t num_classes, int32_t num_iters, const double* init_gamma, int32_t cgmm_init,
+                      int32_t update_alpha, const int32_t* permu_plan, int32_t R, float* masks, uint32_t* status,
+                      void* stream);
+
+/*
+ * The same estimator for a caller that brings its own STFT -- the reference's
+ * CacgmmTrainer(obs, num_classes, gamma, cgmm_init, update_alpha).train(num_iters) signature
+ * (cluster.py:468-535).  Plan-free; scratch is stream-ordered (cudaMallocAsync).
+ *   stft   c64 [B][C][F][T]; other arguments as for setk_cacgmm_masks; any F, T >= 1.
+ */
+int setk_cacgmm_stft(const void* stft, int32_t B, int32_t C, int32_t F, int32_t T, int32_t num_classes,
+                     int32_t num_iters, const double* init_gamma, int32_t cgmm_init, int32_t update_alpha,
+                     const int32_t* permu_plan, int32_t R, float* masks, uint32_t* status, void* stream);
+
+/*
+ * permu_aligner(masks) (cluster.py:48-91) for a batch of fp64 masks: per utterance, the features
+ * are the masks normalised over its own frames; every plan row (iters, lo, hi) re-orders the
+ * classes of each bin in [lo, hi) to the best permutation against the band's centroid, up to
+ * `iters` times or until no bin moves.  Exact score ties keep the current order.
+ *   masks    f64 [B][K][T][F]        n_frames  i32 [B] device, or NULL (every utterance has T)
+ *   plan     host i32 [R][3] as for setk_cacgmm_masks, 1 <= R <= SETK_PERMU_MAX_ROWS
+ *   out      f32 [B][K][T][F] the masks gathered through the mapping, 0 past each n_frames
+ *   mapping  i32 [B][K][F] or NULL: source class of slot k in bin f
+ * Plan-free.  SETK_EINVAL for a null buffer, K outside 2..4, B, T or F < 1, or a bad plan row;
+ * SETK_EUNSUPPORTED when F is too large for the per-bin tables in shared memory.
+ */
+int setk_permu_align(const double* masks, const int32_t* n_frames, int32_t B, int32_t K, int32_t T, int32_t F,
+                     const int32_t* plan, int32_t R, float* out, int32_t* mapping, void* stream);
+
 /*
  * WPE dereverberation of a multichannel STFT: libs/wpe.py wpe(reverb, taps, delay,
  * context, num_iters) (scripts/sptk/libs/wpe.py:82-110 with 14-79; driven by

@@ -120,6 +120,14 @@ _PROTOTYPES = {
                                 c_void_p, c_void_p]),
     "setk_cgmm_stft": (c_int, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32,
                                c_int32, c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),
+    "setk_cacgmm_masks": (c_int, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32,
+                                  c_void_p, c_int32, c_int32, c_void_p, c_int32, c_void_p, c_void_p,
+                                  c_void_p]),
+    "setk_cacgmm_stft": (c_int, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
+                                 c_void_p, c_int32, c_int32, c_void_p, c_int32, c_void_p, c_void_p,
+                                 c_void_p]),
+    "setk_permu_align": (c_int, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p,
+                                 c_int32, c_void_p, c_void_p, c_void_p]),
     "setk_wpe_stft": (c_int, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
                               c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
     "setk_wpe_step": (c_int, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,

@@ -502,6 +502,103 @@ int setk_cgmm_stft(const void* stft, int32_t B, int32_t C, int32_t F, int32_t T,
   });
 }
 
+// plan rows (iterations, lo, hi) of the permutation aligner: 0 <= lo < hi <= F, iterations >= 0;
+// NULL or R = 0 (no alignment) only when `required` is false
+static int check_permu_plan(const char* who, const int32_t* plan, int R, int F, bool required) {
+  if (!plan || R == 0) return required ? fail(SETK_EINVAL, "%s: empty alignment plan", who) : SETK_OK;
+  if (R < 0 || R > SETK_PERMU_MAX_ROWS)
+    return fail(SETK_EINVAL, "%s: %d plan rows outside [1, %d]", who, R, SETK_PERMU_MAX_ROWS);
+  for (int r = 0; r < R; ++r) {
+    const int it = plan[3 * r], lo = plan[3 * r + 1], hi = plan[3 * r + 2];
+    if (it < 0 || lo < 0 || lo >= hi || hi > F)
+      return fail(SETK_EINVAL, "%s: plan row %d (%d, %d, %d) needs iterations >= 0 and 0 <= lo < hi <= F = %d",
+                  who, r, it, lo, hi, F);
+  }
+  return SETK_OK;
+}
+
+// the checks every CACGMM / alignment entry point shares: class count, start, plan rows over F bins
+static int check_cacgmm(const char* who, int C, int K, int num_iters, const double* init_gamma, int cgmm_init,
+                        const int32_t* plan, int R, int F) {
+  if (K < 2 || K > 4) return fail(SETK_EINVAL, "%s: num_classes %d outside 2..4", who, K);
+  if (C < 2) return fail(SETK_EINVAL, "%s: %d channel(s), the CACGMM needs 2 or more", who, C);
+  if (num_iters < 0) return fail(SETK_EINVAL, "%s: num_iters %d", who, num_iters);
+  if (!init_gamma && !(cgmm_init && K == 2))
+    return fail(SETK_EINVAL, "%s: a NULL init_gamma needs cgmm_init with 2 classes", who);
+  return check_permu_plan(who, plan, R, F, false);
+}
+
+int setk_cacgmm_masks(setk_plan_t* pl, const float* audio, const int32_t* n_samples, int32_t B, int32_t N,
+                      int32_t num_classes, int32_t num_iters, const double* init_gamma, int32_t cgmm_init,
+                      int32_t update_alpha, const int32_t* permu_plan, int32_t R, float* masks, uint32_t* status,
+                      void* stream) {
+  int rc = check_batch(pl, B, N, "setk_cacgmm_masks");
+  if (rc) return rc;
+  if (!audio || !masks) return fail(SETK_EINVAL, "setk_cacgmm_masks: null buffer");
+  const Geometry& g = pl->geo;
+  rc = check_cacgmm("setk_cacgmm_masks", g.C, num_classes, num_iters, init_gamma, cgmm_init, permu_plan, R, g.F);
+  if (rc) return rc;
+  if (!stft_spill_supported(g))
+    return fail(SETK_EUNSUPPORTED, "setk_cacgmm_masks: needs n_fft 512 or 1024 (got %d, hop %d)", g.n_fft, g.hop);
+  const int T = frames_of(N, g.n_fft, g.hop, g.pad);
+  if (T < 1) return fail(SETK_ESHAPE, "setk_cacgmm_masks: no frame in %d samples", N);
+  if (permu_plan && R > 0 && permu_scratch_bytes(B, num_classes, T, g.F) < 0)
+    return fail(SETK_EUNSUPPORTED, "setk_cacgmm_masks: %d bins exceed the aligner's shared memory", g.F);
+  const int P = bin_pitch(g.F);
+  CgCtx ctx;
+  ctx.geo = g; ctx.sm_count = pl->sm_count;
+  cudaError_t e = ensure(&pl->d_cgmm_ws, &pl->cgmm_ws_bytes, cacgmm_workspace_bytes(&ctx, B, T, num_classes, P));
+  if (e != cudaSuccess) return cuda_fail(e, "setk_cacgmm_masks(workspace)");
+  rc = stft_to_bin_major(pl, audio, n_samples, B, N, T, nullptr, stream, "setk_cacgmm_masks(workspace)",
+                         "setk_cacgmm_masks");
+  if (rc) return rc;
+  e = run_cacgmm(&ctx, pl->d_stft_ws, P, pl->d_cgmm_ws, n_samples, B, N, T, num_classes, num_iters, init_gamma,
+                 cgmm_init, update_alpha, permu_plan, permu_plan ? R : 0, masks, status, stream);
+  return done(e, "setk_cacgmm_masks");
+}
+
+int setk_cacgmm_stft(const void* stft, int32_t B, int32_t C, int32_t F, int32_t T, int32_t num_classes,
+                     int32_t num_iters, const double* init_gamma, int32_t cgmm_init, int32_t update_alpha,
+                     const int32_t* permu_plan, int32_t R, float* masks, uint32_t* status, void* stream) {
+  if (!stft || !masks) return fail(SETK_EINVAL, "setk_cacgmm_stft: null buffer");
+  if (B < 1 || B > 65535 || F < 1 || T < 1 || C < 1 || C > SETK_MAX_CHANNELS)
+    return fail(SETK_ESHAPE, "setk_cacgmm_stft: bad shape B=%d C=%d F=%d T=%d", B, C, F, T);
+  int rc = check_cacgmm("setk_cacgmm_stft", C, num_classes, num_iters, init_gamma, cgmm_init, permu_plan, R, F);
+  if (rc) return rc;
+  if (permu_plan && R > 0 && permu_scratch_bytes(B, num_classes, T, F) < 0)
+    return fail(SETK_EUNSUPPORTED, "setk_cacgmm_stft: %d bins exceed the aligner's shared memory", F);
+  CgCtx ctx;
+  // frames are given, not derived from samples: a geometry whose frame count never limits
+  ctx.geo.C = C; ctx.geo.F = F; ctx.geo.n_fft = 2; ctx.geo.log2n = 1; ctx.geo.hop = 1; ctx.geo.pad = 0;
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&ctx.sm_count, cudaDevAttrMultiProcessorCount, dev);
+  if (e != cudaSuccess) return cuda_fail(e, "setk_cacgmm_stft(device)");
+  return with_bin_major(stft, B, C, F, T, cacgmm_workspace_bytes(&ctx, B, T, num_classes, bin_pitch(F)), stream,
+                        "setk_cacgmm_stft(workspace)", "setk_cacgmm_stft", [&](float2* X, int P, double* ws) {
+    return run_cacgmm(&ctx, X, P, ws, nullptr, B, /*N=*/T + 1, T, num_classes, num_iters, init_gamma, cgmm_init,
+                      update_alpha, permu_plan, permu_plan ? R : 0, masks, status, stream);
+  });
+}
+
+int setk_permu_align(const double* masks, const int32_t* n_frames, int32_t B, int32_t K, int32_t T, int32_t F,
+                     const int32_t* plan, int32_t R, float* out, int32_t* mapping, void* stream) {
+  if (!masks || !out) return fail(SETK_EINVAL, "setk_permu_align: null buffer");
+  if (K < 2 || K > 4) return fail(SETK_EINVAL, "setk_permu_align: num_classes %d outside 2..4", K);
+  if (B < 1 || T < 1 || F < 1) return fail(SETK_EINVAL, "setk_permu_align: bad shape B=%d T=%d F=%d", B, T, F);
+  int rc = check_permu_plan("setk_permu_align", plan, R, F, true);
+  if (rc) return rc;
+  const long long sb = permu_scratch_bytes(B, K, T, F);
+  if (sb < 0) return fail(SETK_EUNSUPPORTED, "setk_permu_align: %d bins exceed the aligner's shared memory", F);
+  PermuArgs a;
+  a.m = masks; a.ld = F; a.n_frames = n_frames; a.n_samples = nullptr; a.N = T + 1;
+  a.g.C = 1; a.g.F = F; a.g.n_fft = 2; a.g.log2n = 1; a.g.hop = 1; a.g.pad = 0;   // T frames unless n_frames
+  a.K = K; a.T = T; a.F = F;
+  return with_scratch((size_t)sb + 256, stream, "setk_permu_align(scratch)", "setk_permu_align", [&](char* ws) {
+    return run_permu_align(a, B, plan, R, reinterpret_cast<double*>(ws), out, mapping, stream);
+  });
+}
+
 static int wpe_entry(const char* who, const void* stft, const void* lambda_enh, int32_t B, int32_t C, int32_t F,
                      int32_t T, int32_t taps, int32_t delay, int32_t context, int32_t num_iters, void* out,
                      float* inv_lambda, uint32_t* status, void* stream) {

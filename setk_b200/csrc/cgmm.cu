@@ -22,6 +22,12 @@
 //                       shared memory: phi_k = max(|y^H R_k^-1 y|, eps)/M, the
 //                       posterior (log-sum-exp shifted), G and W for the next pass.
 // All arithmetic after the complex64 STFT is fp64, as in the reference.
+//
+// The CACGMM (cluster.py:290-393, 468-535) runs the same three passes on the unit-norm
+// observations z = y / n, n = max(|y|_2, eps), without a normalised copy of X: since
+// z z^H = y y^H / n^2 and z^H B^-1 z = y^H B^-1 y / n^2, the covariance pass takes the weight
+// W = gamma M / (kappa n^2), kappa = max(|y^H B^-1 y| / n^2, eps), which the E-step writes
+// (ACG = true), and the start writes W = gamma M / n^2 (cacgmm_import_kernel).
 #include "async_copy.cuh"
 #include "common.cuh"
 #include "jacobi_coop.cuh"
@@ -330,8 +336,9 @@ struct CgmmEstepArgs {
   double* G; double* W;      // [B][K][T][P]
 };
 
-// BL bins x (256 / BL) frame lanes per CTA; R^-1 of the BL bins in shared memory
-template <int C, int K, int BL>
+// BL bins x (256 / BL) frame lanes per CTA; R^-1 of the BL bins in shared memory.
+// ACG: the CACGMM's log-pdf and weight (cluster.py:311-337, 367-393) instead of the CGMM's.
+template <int C, int K, int BL, bool ACG>
 __global__ void __launch_bounds__(256) cgmm_estep_kernel(CgmmEstepArgs a) {
   SETK_DYN_SMEM(double, rs);                 // [K][C*C][BL]
   constexpr int L = 256 / BL, CC = C * C;
@@ -361,7 +368,9 @@ __global__ void __launch_bounds__(256) cgmm_estep_kernel(CgmmEstepArgs a) {
   }
   const long long P = a.P;
   const double* r = rs + bl;
-  constexpr int FR = 2;                      // frames in flight per thread: R^-1 is read once for both
+  // frames in flight per thread: R^-1 is read once for both.  ACG keeps one: its n^2 per frame would
+  // otherwise push most C >= 5 instantiations further into local memory.
+  constexpr int FR = ACG ? 1 : 2;
   constexpr bool PF = C <= 8;                // prefetch the next pair of frames (registers allow it)
   float2 nx[FR][PF ? C : 1];
   auto fetch = [&](int t) {
@@ -429,10 +438,23 @@ __global__ void __launch_bounds__(256) cgmm_estep_kernel(CgmmEstepArgs a) {
       const int tt = t + u * L;
       if (tt >= t_end) break;
       double phi[K], lp[K], mx = -1.0e300;
+      double n2 = 1.0;                                               // |y|^2 floored (ACG)
+      if constexpr (ACG) {
+        n2 = 0.0;
+#pragma unroll
+        for (int c = 0; c < C; ++c) n2 += yr[u][c] * yr[u][c] + yi[u][c] * yi[u][c];
+        const double n = fmax(sqrt(n2), SETK_EPS32_D);              // cluster.py:39-45
+        n2 = n * n;
+      }
 #pragma unroll
       for (int k = 0; k < K; ++k) {
-        phi[k] = fmax(fabs(q[u][k]), SETK_EPS32_D) / (double)C;      // cluster.py:203-206
-        lp[k] = -(double)C * log(phi[k]) - ld[k];                    // cluster.py:228-229
+        if constexpr (ACG) {
+          phi[k] = fmax(fabs(q[u][k]) / n2, SETK_EPS32_D);           // kappa, cluster.py:326-329
+          lp[k] = -(double)C * log(phi[k]) - ld[k];                  // cluster.py:331-332
+        } else {
+          phi[k] = fmax(fabs(q[u][k]), SETK_EPS32_D) / (double)C;    // cluster.py:203-206
+          lp[k] = -(double)C * log(phi[k]) - ld[k];                  // cluster.py:228-229
+        }
         mx = fmax(mx, lp[k]);
       }
       double den = 0.0;
@@ -444,7 +466,8 @@ __global__ void __launch_bounds__(256) cgmm_estep_kernel(CgmmEstepArgs a) {
         const double gm = lp[k] / den;
         const long long o = (((long long)b * K + k) * a.T + tt) * P + bin;
         a.G[o] = gm;
-        a.W[o] = gm * (double)C / phi[k];
+        if constexpr (ACG) a.W[o] = gm * (double)C / (phi[k] * n2);  // cluster.py:305-308 on z = y / n
+        else a.W[o] = gm * (double)C / phi[k];
       }
     }
   }
@@ -460,6 +483,32 @@ __global__ void cgmm_import_kernel(const float* __restrict__ gin, int B, int K, 
   const double v = gin[idx];
   G[row * P + f] = v;
   W[row * P + f] = v;
+}
+
+// CACGMM start, thread per (b, t, f) (cluster.py:508-518): init_gamma f64 [B][K][T][F] -> G = gamma,
+// W = gamma M / n^2 (the kernel term is ones); without it (cgmm_init) G = 1, W = 1 / n^2, so that
+// the covariance pass forms sum_t z z^H / T_b (cluster.py:495-505).  n as in the E-step.
+__global__ void cacgmm_import_kernel(const double* __restrict__ gin, const float2* __restrict__ X, int P, int C,
+                                     int B, int K, int T, int F, double* __restrict__ G, double* __restrict__ W) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)B * T * F) return;
+  const int f = (int)(idx % F);
+  const long long bt = idx / F;               // b * T + t
+  const int b = (int)(bt / T), t = (int)(bt - (long long)b * T);
+  const float2* x = X + bt * C * P + f;
+  double n2 = 0.0;
+  for (int c = 0; c < C; ++c) {
+    const double re = x[(long long)c * P].x, im = x[(long long)c * P].y;
+    n2 += re * re + im * im;
+  }
+  const double n = fmax(sqrt(n2), SETK_EPS32_D);
+  n2 = n * n;
+  for (int k = 0; k < K; ++k) {
+    const long long row = ((long long)b * K + k) * T + t;
+    const double g = gin ? gin[row * F + f] : 1.0;
+    G[row * P + f] = g;
+    W[row * P + f] = gin ? g * (double)C / n2 : 1.0 / n2;
+  }
 }
 
 // G -> masks f32 [B][K][T][F]; frames past the utterance's own count are zero
@@ -622,12 +671,12 @@ static cudaError_t cgmm_factor(const CgCtx* pl, const CgmmWorkspace& w, int iden
   }
 }
 
-template <int C, int K>
+template <int C, int K, bool ACG>
 static cudaError_t cgmm_estep_t(const CgCtx* pl, CgmmEstepArgs a, int B, void* stream) {
   constexpr int BL = C <= 8 ? 64 : 16;
   const size_t smem = sizeof(double) * K * C * C * BL;
 #ifndef SETK_EMU
-  cudaError_t e = cudaFuncSetAttribute(cgmm_estep_kernel<C, K, BL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  cudaError_t e = cudaFuncSetAttribute(cgmm_estep_kernel<C, K, BL, ACG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        (int)smem);
   if (e != cudaSuccess) return e;
 #endif
@@ -637,19 +686,20 @@ static cudaError_t cgmm_estep_t(const CgCtx* pl, CgmmEstepArgs a, int B, void* s
   if (chunks > a.T) chunks = a.T;
   a.frames_per_chunk = (a.T + chunks - 1) / chunks;
   chunks = (a.T + a.frames_per_chunk - 1) / a.frames_per_chunk;
-  return launch(cgmm_estep_kernel<C, K, BL>, dim3(chunks * nbb, B), dim3(256), smem, stream, false, a);
+  return launch(cgmm_estep_kernel<C, K, BL, ACG>, dim3(chunks * nbb, B), dim3(256), smem, stream, false, a);
 }
 
-template <int C>
+template <int C, bool ACG>
 static cudaError_t cgmm_estep_c(const CgCtx* pl, const CgmmEstepArgs& a, int B, int K, void* stream) {
   switch (K) {
-    case 2: return cgmm_estep_t<C, 2>(pl, a, B, stream);
-    case 3: return cgmm_estep_t<C, 3>(pl, a, B, stream);
-    case 4: return cgmm_estep_t<C, 4>(pl, a, B, stream);
+    case 2: return cgmm_estep_t<C, 2, ACG>(pl, a, B, stream);
+    case 3: return cgmm_estep_t<C, 3, ACG>(pl, a, B, stream);
+    case 4: return cgmm_estep_t<C, 4, ACG>(pl, a, B, stream);
     default: return cudaErrorInvalidValue;
   }
 }
 
+template <bool ACG>
 static cudaError_t cgmm_estep(const CgCtx* pl, const float2* X, int P, const CgmmWorkspace& w,
                               const int* n_samples, int B, int N, int T, int K, void* stream) {
   CgmmEstepArgs a;
@@ -659,7 +709,7 @@ static cudaError_t cgmm_estep(const CgCtx* pl, const float2* X, int P, const Cgm
   a.T = T; a.frames_per_chunk = T;
   a.G = w.G; a.W = w.W;
   switch (pl->geo.C) {
-#define SETK_CASE(k) case k: return cgmm_estep_c<k>(pl, a, B, K, stream);
+#define SETK_CASE(k) case k: return cgmm_estep_c<k, ACG>(pl, a, B, K, stream);
     SETK_CASE(1) SETK_CASE(2) SETK_CASE(3) SETK_CASE(4) SETK_CASE(5) SETK_CASE(6) SETK_CASE(7) SETK_CASE(8)
     SETK_CASE(9) SETK_CASE(10) SETK_CASE(11) SETK_CASE(12) SETK_CASE(13) SETK_CASE(14) SETK_CASE(15) SETK_CASE(16)
 #undef SETK_CASE
@@ -689,13 +739,60 @@ cudaError_t run_cgmm(const CgCtx* pl, const float2* X, int P, double* ws, const 
   }
   e = cgmm_cov(pl, X, P, w, uniform, n_samples, B, N, T, K, stream);
   if (e == cudaSuccess) e = cgmm_factor(pl, w, uniform ? 1 : -1, 0, n_samples, B, N, T, K, status, stream);
-  if (e == cudaSuccess) e = cgmm_estep(pl, X, P, w, n_samples, B, N, T, K, stream);
+  if (e == cudaSuccess) e = cgmm_estep<false>(pl, X, P, w, n_samples, B, N, T, K, stream);
   for (int it = 0; it < num_iters && e == cudaSuccess; ++it) {
     e = cgmm_cov(pl, X, P, w, false, n_samples, B, N, T, K, stream);
     if (e == cudaSuccess) e = cgmm_factor(pl, w, -1, update_alpha, n_samples, B, N, T, K, status, stream);
-    if (e == cudaSuccess) e = cgmm_estep(pl, X, P, w, n_samples, B, N, T, K, stream);
+    if (e == cudaSuccess) e = cgmm_estep<false>(pl, X, P, w, n_samples, B, N, T, K, stream);
   }
   if (e != cudaSuccess) return e;
+  const long long n = (long long)B * K * T * g.F;
+  return launch(cgmm_export_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, stream, true,
+                (const double*)w.G, n_samples, N, g, B, K, T, P, masks);
+}
+
+size_t cacgmm_workspace_bytes(const CgCtx* pl, int B, int T, int K, int P) {
+  return cgmm_workspace_bytes(pl, B, T, K, P) + sizeof(double) * (size_t)B * K * T;   // + aligner centroids
+}
+
+// CacgmmTrainer(obs, K, gamma, cgmm_init=..., update_alpha=...).train(num_iters) (cluster.py:468-535)
+// over the workspace X, then permu_aligner (cluster.py:48-91) on the fp64 posteriors when R > 0.
+cudaError_t run_cacgmm(const CgCtx* pl, const float2* X, int P, double* ws, const int* n_samples, int B, int N,
+                       int T, int K, int num_iters, const double* init_gamma, int cgmm_init, int update_alpha,
+                       const int* permu_rows, int R, float* masks, unsigned* status, void* stream) {
+  const Geometry& g = pl->geo;
+  const CgmmWorkspace w = cgmm_carve(pl, ws, B, T, K, P);
+  cudaError_t e;
+  {  // alpha = 1 / K  (cluster.py:485)
+    const long long n = (long long)B * K * g.F;
+    e = launch(cgmm_fill_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, stream, true, w.alpha, n,
+               1.0 / (double)K);
+    if (e != cudaSuccess) return e;
+  }
+  const bool from_cgmm = cgmm_init && K == 2;
+  {
+    const long long n = (long long)B * T * g.F;
+    e = launch(cacgmm_import_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, stream, true,
+               from_cgmm ? nullptr : init_gamma, X, P, g.C, B, K, T, g.F, w.G, w.W);
+    if (e != cudaSuccess) return e;
+  }
+  if (from_cgmm) {   // B_0 = sum_t z z^H / T, B_1 = I, then one E-step (cluster.py:495-506)
+    e = cgmm_cov(pl, X, P, w, false, n_samples, B, N, T, K, stream);
+    if (e == cudaSuccess) e = cgmm_factor(pl, w, 1, 0, n_samples, B, N, T, K, status, stream);
+    if (e == cudaSuccess) e = cgmm_estep<true>(pl, X, P, w, n_samples, B, N, T, K, stream);
+  }
+  for (int it = 0; it < num_iters && e == cudaSuccess; ++it) {
+    e = cgmm_cov(pl, X, P, w, false, n_samples, B, N, T, K, stream);
+    if (e == cudaSuccess) e = cgmm_factor(pl, w, -1, update_alpha, n_samples, B, N, T, K, status, stream);
+    if (e == cudaSuccess) e = cgmm_estep<true>(pl, X, P, w, n_samples, B, N, T, K, stream);
+  }
+  if (e != cudaSuccess) return e;
+  if (R > 0) {
+    PermuArgs a;
+    a.m = w.G; a.ld = P; a.n_frames = nullptr; a.n_samples = n_samples; a.N = N; a.g = g;
+    a.K = K; a.T = T; a.F = g.F;
+    return run_permu_align(a, B, permu_rows, R, w.alpha + (size_t)B * K * g.F, masks, nullptr, stream);
+  }
   const long long n = (long long)B * K * T * g.F;
   return launch(cgmm_export_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, stream, true,
                 (const double*)w.G, n_samples, N, g, B, K, T, P, masks);

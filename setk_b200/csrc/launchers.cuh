@@ -87,6 +87,23 @@ size_t cgmm_workspace_bytes(const CgCtx* pl, int B, int T, int K, int P);
 cudaError_t run_cgmm(const CgCtx* pl, const float2* X, int P, double* ws, const int* n_samples, int B, int N,
                      int T, int K, int num_iters, const float* init_gamma, int update_alpha, float* masks,
                      unsigned* status, void* stream);
+size_t cacgmm_workspace_bytes(const CgCtx* pl, int B, int T, int K, int P);
+cudaError_t run_cacgmm(const CgCtx* pl, const float2* X, int P, double* ws, const int* n_samples, int B, int N,
+                       int T, int K, int num_iters, const double* init_gamma, int cgmm_init, int update_alpha,
+                       const int* permu_rows, int R, float* masks, unsigned* status, void* stream);
+
+// ---- permu.cu: frequency permutation alignment of K-class masks ----
+struct PermuArgs {
+  const double* m; int ld;       // posteriors [B][K][T][ld], bins [0, F) of each row
+  const int* n_frames;           // [B] frames per utterance, or null: from n_samples / N and g
+  const int* n_samples; int N; Geometry g;
+  int K, T, F;
+};
+// bytes of global centroid scratch a call needs (0 when the centroids fit in shared memory); -1 when
+// the per-bin tables alone exceed shared memory
+long long permu_scratch_bytes(int B, int K, int T, int F);
+cudaError_t run_permu_align(const PermuArgs& a, int B, const int* rows_host, int R, double* scratch,
+                            float* out, int* mapping, void* stream);
 
 // ---- wpe.cu (with auxiva.cuh): fp64 per-bin iterative front ends ----
 bool wpe_supported(int C, int T, int taps, int delay, int ctx);

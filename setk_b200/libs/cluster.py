@@ -1,8 +1,9 @@
 """
-setk_b200.libs.cluster -- GPU mirror of the reference's CGMM trainer
-(scripts/sptk/libs/cluster.py:396-465, with the model classes 94-287 behind it).
+setk_b200.libs.cluster -- GPU mirror of the reference's CGMM and CACGMM trainers
+(scripts/sptk/libs/cluster.py:396-465 and 468-535, with the model classes 94-393 behind them).
 
     trainer = CgmmTrainer(obs, num_classes, gamma=None, cgmm=None, update_alpha=False)
+    trainer = CacgmmTrainer(obs, num_classes, gamma=None, cacgmm=None, cgmm_init=False, update_alpha=True)
     gamma = trainer.train(num_iters)          # K x F x T posteriors
 
 Same constructor / method names, argument meaning and array axes as the
@@ -22,7 +23,12 @@ Differences from the reference, all deliberate:
   * `cgmm=<pickle path>` (resume) raises: the reference opens the pickle in text
     mode, which cannot work under Python 3 (cluster.py:455-457).
   * the per-iteration log value Q is not computed.
-  * the CACGMM trainer (cluster.py:468-560) is outside SURVEY.md §8.
+  * CacgmmTrainer runs setk_cacgmm_stft (csrc/cgmm.cu with ACG = true) and draws its random
+    start with np.random.uniform in the constructor, as the reference does, so np.random.seed
+    reproduces a reference run.  Its start is float64 and its masks come back float32;
+    `cacgmm=<pickle path>` raises like `cgmm=`; a non-converged eigen-iteration raises
+    numpy.linalg.LinAlgError, as the reference's eigh would.
+  * permu_aligner below is host numpy; plan.permu_align is its device form.
 """
 import numpy as np
 import torch
@@ -32,16 +38,10 @@ from .utils import EPSILON, default_device, get_logger
 
 logger = get_logger(__name__)
 
-__all__ = ["CgmmTrainer", "permu_aligner", "norm_observation", "supported_plan"]
+__all__ = ["CgmmTrainer", "CacgmmTrainer", "permu_aligner", "norm_observation", "supported_plan"]
 
 # frequency sub-band schedule of the permutation aligner: (iterations, first bin, end bin)
-supported_plan = {
-    257: [(20, 70, 170), (2, 90, 190), (2, 50, 150), (2, 110, 210), (2, 30, 130), (2, 130, 230),
-          (2, 0, 110), (2, 150, 257)],
-    513: [(20, 100, 200), (2, 120, 220), (2, 80, 180), (2, 140, 240), (2, 60, 160), (2, 160, 260),
-          (2, 40, 140), (2, 180, 280), (2, 0, 120)] +
-         [(2, lo, lo + 100) for lo in range(200, 400, 20)] + [(2, 400, 513)],
-}
+supported_plan = _plan.PERMU_PLANS
 
 
 def norm_observation(mat, axis=-1, eps=EPSILON):
@@ -98,6 +98,21 @@ def permu_aligner(masks, transpose=False):
     return out
 
 
+def _complex_obs(obs, who):
+    """obs M x F x T (or B x M x F x T) -> (complex64 B x M x F x T on a CUDA device, was numpy, batched)"""
+    numpy = isinstance(obs, np.ndarray)
+    obs = torch.as_tensor(obs)
+    if not torch.is_complex(obs):
+        raise RuntimeError(f"{who} expects a complex STFT, M x F x T")
+    batched = obs.dim() == 4
+    if obs.dim() == 3:
+        obs = obs[None]
+    if obs.dim() != 4:
+        raise RuntimeError(f"Expect M x F x T observations, got {tuple(obs.shape)}")
+    dev = obs.device if obs.device.type == "cuda" else default_device()
+    return obs.to(dev).to(torch.complex64).contiguous(), numpy, batched
+
+
 class CgmmTrainer(object):
     """
     CGMM trainer (cluster.py:396-465).
@@ -110,17 +125,8 @@ class CgmmTrainer(object):
         if cgmm is not None:
             raise NotImplementedError("resuming from a pickled Cgmm is not supported "
                                       "(broken in the reference: text-mode pickle, cluster.py:455)")
-        self._numpy = isinstance(obs, np.ndarray)
-        obs = torch.as_tensor(obs)
-        if not torch.is_complex(obs):
-            raise RuntimeError("CgmmTrainer expects a complex STFT, M x F x T")
-        self._batched = obs.dim() == 4
-        if obs.dim() == 3:
-            obs = obs[None]
-        if obs.dim() != 4:
-            raise RuntimeError(f"Expect M x F x T observations, got {tuple(obs.shape)}")
-        dev = obs.device if obs.device.type == "cuda" else default_device()
-        self.obs = obs.to(dev).to(torch.complex64).contiguous()
+        self.obs, self._numpy, self._batched = _complex_obs(obs, "CgmmTrainer")
+        dev = self.obs.device
         B, M, F, T = self.obs.shape
         self.num_classes = int(num_classes)
         self.update_alpha = bool(update_alpha)
@@ -153,6 +159,64 @@ class CgmmTrainer(object):
         bad = status.nonzero().flatten().tolist()
         if bad:
             raise RuntimeError(f"CGMM: eigen-iteration did not converge for batch entries {bad}")
+        gamma = masks.transpose(-1, -2)                              # K x F x T like the reference
+        if not self._batched:
+            gamma = gamma[0]
+        self.gamma = gamma.cpu().numpy() if self._numpy else gamma
+        return self.gamma
+
+
+class CacgmmTrainer(object):
+    """
+    CACGMM trainer (cluster.py:468-535).
+        obs        mixture STFT, M x F x T complex (or B x M x F x T for a batch)
+        gamma      starting posteriors K x F x T (B x K x F x T), used as given; None draws
+                   np.random.uniform(size=[K, F, T]) here (per utterance, in batch order) and
+                   normalises it over classes, unless cgmm_init with 2 classes
+        cgmm_init  with 2 classes: the start B_0 = sum_t z z^H / T, B_1 = I and one E-step
+    """
+
+    def __init__(self, obs, num_classes, gamma=None, cacgmm=None, cgmm_init=False, update_alpha=True):
+        if cacgmm is not None:
+            raise NotImplementedError("resuming from a pickled Cacgmm is not supported "
+                                      "(broken in the reference: text-mode pickle, cluster.py:520-522)")
+        self.obs, self._numpy, self._batched = _complex_obs(obs, "CacgmmTrainer")
+        B, M, F, T = self.obs.shape
+        self.num_classes = K = int(num_classes)
+        self.update_alpha = bool(update_alpha)
+        self.cgmm_init = bool(cgmm_init) and K == 2
+        logger.info(f"CACGMM instance: F = {F:d}, T = {T:}, M = {M}")
+        self._init = None
+        if gamma is not None:
+            g = torch.as_tensor(gamma).to(self.obs.device).to(torch.float64)
+            if not self._batched:
+                g = g[None]
+            if tuple(g.shape) != (B, K, F, T):
+                raise RuntimeError(f"gamma must be K x F x T = {(K, F, T)}, got {tuple(g.shape[1:])}")
+            self._init = g.transpose(-1, -2).contiguous()            # library layout K x T x F
+        elif self.cgmm_init:
+            logger.info("Using cgmm init for num_classes = 2")
+        else:
+            draws = []
+            for _ in range(B):                                        # cluster.py:509-512
+                g = np.random.uniform(size=[K, F, T])
+                draws.append(np.transpose(g / np.sum(g, 0, keepdims=True), (0, 2, 1)))
+            self._init = torch.from_numpy(np.ascontiguousarray(np.stack(draws))).to(self.obs.device)
+            logger.info(f"Random initialized, num_classes = {K}")
+        self._iters = 0
+        self.gamma = None
+
+    def train(self, num_iters):
+        """
+        EM iterations; returns the posteriors K x F x T.  Calling it again continues: the run is
+        deterministic, so it is redone with the accumulated count.
+        """
+        self._iters += int(num_iters)
+        masks, status = _plan.cacgmm_from_stft(self.obs, self.num_classes, self._iters, init_gamma=self._init,
+                                               cgmm_init=self.cgmm_init, update_alpha=self.update_alpha)
+        bad = status.nonzero().flatten().tolist()
+        if bad:
+            raise np.linalg.LinAlgError(f"CACGMM: eigen-iteration did not converge for batch entries {bad}")
         gamma = masks.transpose(-1, -2)                              # K x F x T like the reference
         if not self._batched:
             gamma = gamma[0]

@@ -211,6 +211,28 @@ class StftPlan(object):
                 _lib.ptr(init_gamma), 1 if update_alpha else 0, _lib.ptr(masks), _lib.ptr(status))
         return masks, status
 
+    def cacgmm_masks(self, audio, num_classes=2, num_iters=50, init_gamma=None, cgmm_init=False,
+                     update_alpha=True, permu_plan=None, n_samples=None):
+        """
+        CACGMM mask estimation from audio (STFT + CacgmmTrainer(...).train(num_iters), cluster.py:468-535),
+        then permu_aligner (cluster.py:48-91) on the fp64 posteriors when `permu_plan` rows (iterations,
+        first bin, end bin) are given (PERMU_PLANS[F] is the reference's).  init_gamma (B,K,T,F) float64, or
+        None with cgmm_init and 2 classes.  Returns (masks (B,K,T,F) float32, status (B,) int32).
+        """
+        audio = self._check_audio(audio)
+        B, C, N = audio.shape
+        T = self.num_frames(N)
+        F = self.num_bins
+        K, rows, rows_p, R = _cacgmm_checks(C, num_classes, num_iters, init_gamma, cgmm_init, permu_plan, F)
+        init_gamma = _arg(init_gamma, self.device, torch.float64, (B, K, T, F), "init_gamma")
+        ns = _arg(n_samples, self.device, torch.int32, (B,), "n_samples")
+        masks = torch.empty((B, K, T, F), dtype=torch.float32, device=self.device)
+        status = torch.zeros((B,), dtype=torch.int32, device=self.device)
+        _launch(self.device, "setk_cacgmm_masks", self._h, _lib.ptr(audio), _lib.ptr(ns), B, N, K, int(num_iters),
+                _lib.ptr(init_gamma), int(bool(cgmm_init)), int(bool(update_alpha)), rows_p, R, _lib.ptr(masks),
+                _lib.ptr(status))
+        return masks, status
+
     def istft(self, enh, n_out=None, norm=None):
         """enh (B,F,T) complex64 -> wave (B,n_out) float32 (inverse_stft)."""
         enh = _arg(enh, self.device, torch.complex64, (None, self.num_bins, None), "enh")
@@ -261,6 +283,94 @@ def cgmm_from_stft(stft, num_classes=2, num_iters=20, init_gamma=None, update_al
     _launch(stft.device, "setk_cgmm_stft", _lib.ptr(stft), B, C, F, T, K, int(num_iters), _lib.ptr(init_gamma),
             1 if update_alpha else 0, _lib.ptr(masks), _lib.ptr(status))
     return masks, status
+
+
+# frequency sub-band schedule of the permutation aligner, per number of bins: rows of (iterations,
+# first bin, end bin) (cluster.py:29-36)
+PERMU_PLANS = {
+    257: [(20, 70, 170), (2, 90, 190), (2, 50, 150), (2, 110, 210), (2, 30, 130), (2, 130, 230),
+          (2, 0, 110), (2, 150, 257)],
+    513: [(20, 100, 200), (2, 120, 220), (2, 80, 180), (2, 140, 240), (2, 60, 160), (2, 160, 260),
+          (2, 40, 140), (2, 180, 280), (2, 0, 120)] +
+         [(2, lo, lo + 100) for lo in range(200, 400, 20)] + [(2, 400, 513)],
+}
+
+
+def _permu_rows(plan, F):
+    """plan rows as a host int32 (R, 3) table: (array, pointer, R); ValueError unless 0 <= lo < hi <= F,
+    iterations >= 0 and 1 <= R <= 64 (SETK_PERMU_MAX_ROWS)."""
+    rows = np.asarray(plan, dtype=np.int64).reshape(-1, 3) if np.size(plan) else np.zeros((0, 3), np.int64)
+    if not 1 <= rows.shape[0] <= 64:
+        raise ValueError(f"an alignment plan has 1..64 rows, got {rows.shape[0]}")
+    bad = (rows[:, 0] < 0) | (rows[:, 1] < 0) | (rows[:, 1] >= rows[:, 2]) | (rows[:, 2] > F)
+    if bad.any():
+        raise ValueError(f"alignment plan row {tuple(rows[bad][0])}: needs iterations >= 0 and "
+                         f"0 <= lo < hi <= F = {F}")
+    a, p = _host_i32(rows)
+    return a, p, rows.shape[0]
+
+
+def _cacgmm_checks(C, num_classes, num_iters, init_gamma, cgmm_init, permu_plan, F):
+    """The arguments setk_cacgmm_* refuse, as ValueError: returns (K, plan table, its pointer, R)."""
+    K = int(num_classes)
+    if not 2 <= K <= 4:
+        raise ValueError(f"CACGMM: num_classes {K} outside 2..4")
+    if C < 2:
+        raise ValueError(f"CACGMM: {C} channel(s), needs 2 or more")
+    if int(num_iters) < 0:
+        raise ValueError(f"CACGMM: num_iters {num_iters} < 0")
+    if init_gamma is None and not (cgmm_init and K == 2):
+        raise ValueError("CACGMM: starting posteriors init_gamma are needed unless cgmm_init with 2 classes")
+    if permu_plan is None:
+        return K, None, None, 0
+    return (K, *_permu_rows(permu_plan, F))
+
+
+def cacgmm_from_stft(stft, num_classes=2, num_iters=50, init_gamma=None, cgmm_init=False, update_alpha=True,
+                     permu_plan=None):
+    """
+    CacgmmTrainer(obs, K, gamma, cgmm_init=..., update_alpha=...).train(num_iters) batched (cluster.py:468-535),
+    then permu_aligner on the fp64 posteriors when `permu_plan` is given.  stft (B,C,F,T) complex64;
+    init_gamma (B,K,T,F) float64 or None (cgmm_init with 2 classes).
+    Returns (masks (B,K,T,F) float32, status (B,) int32).
+    """
+    stft = _arg(stft, None, torch.complex64, (None,) * 4, "stft")
+    B, C, F, T = stft.shape
+    K, rows, rows_p, R = _cacgmm_checks(C, num_classes, num_iters, init_gamma, cgmm_init, permu_plan, F)
+    init_gamma = _arg(init_gamma, stft.device, torch.float64, (B, K, T, F), "init_gamma")
+    masks = torch.empty((B, K, T, F), dtype=torch.float32, device=stft.device)
+    status = torch.zeros((B,), dtype=torch.int32, device=stft.device)
+    _launch(stft.device, "setk_cacgmm_stft", _lib.ptr(stft), B, C, F, T, K, int(num_iters), _lib.ptr(init_gamma),
+            int(bool(cgmm_init)), int(bool(update_alpha)), rows_p, R, _lib.ptr(masks), _lib.ptr(status))
+    return masks, status
+
+
+def permu_align(masks, n_frames=None, plan=None):
+    """
+    permu_aligner(masks) (cluster.py:48-91) on the device: masks K x T x F (or a batch B x K x T x F),
+    aligned in float64; n_frames (B,) frames of each utterance of a batch (None: T); plan the sub-band
+    rows (None: PERMU_PLANS[F], ValueError for another F, as the reference).  Returns (the masks gathered
+    through the mapping, float32, same shape; the mapping K x F (B x K x F) int32, source class of slot k).
+    """
+    masks = torch.as_tensor(masks)
+    if masks.dim() not in (3, 4):
+        raise RuntimeError("Expect 3D TF-masks, K x T x F or K x F x T")
+    single = masks.dim() == 3
+    masks = _arg(masks[None] if single else masks, None, torch.float64, (None,) * 4, "masks")
+    B, K, T, F = masks.shape
+    if plan is None:
+        if F not in PERMU_PLANS:
+            raise ValueError(f"Unsupported num_bins: {F}")
+        plan = PERMU_PLANS[F]
+    if not 2 <= K <= 4:
+        raise ValueError(f"permu_align: {K} classes outside 2..4")
+    rows, rows_p, R = _permu_rows(plan, F)
+    nf = _arg(n_frames, masks.device, torch.int32, (B,), "n_frames")
+    out = torch.empty((B, K, T, F), dtype=torch.float32, device=masks.device)
+    mapping = torch.empty((B, K, F), dtype=torch.int32, device=masks.device)
+    _launch(masks.device, "setk_permu_align", _lib.ptr(masks), _lib.ptr(nf), B, K, T, F, rows_p, R, _lib.ptr(out),
+            _lib.ptr(mapping))
+    return (out[0], mapping[0]) if single else (out, mapping)
 
 
 def wpe_from_stft(stft, taps=10, delay=3, context=1, num_iters=3):
