@@ -7,8 +7,9 @@
  *
  * and the front ends around it: CGMM masks, WPE / WPD, spatial features, sound
  * source localisation, AuxIVA blind source separation, iMCRA / OM-LSA
- * noise suppression, image-method room impulse responses, mixture simulation
- * and the separation metrics (BSS-Eval SDR / SIR / SAR, SI-SNR).
+ * noise suppression, image-method room impulse responses, mixture simulation,
+ * the separation metrics (BSS-Eval SDR / SIR / SAR, SI-SNR) and spectral features
+ * (magnitude / power / log spectrogram, log-mel filterbank).
  *
  * Every entry point below replaces one reference interface; the citation is
  * the reference file:line (paths relative to the reference tree).  The Python
@@ -140,6 +141,35 @@ int setk_num_bins(const setk_plan_t* plan);
  * stft_out c64 [B][C][F][T], T = setk_num_frames(plan, N). */
 int setk_stft(setk_plan_t* plan, const float* audio, const int32_t* n_samples,
               int32_t B, int32_t N, void* stft_out, void* stream);
+
+/* Spectral features, compute_spectrogram.py:19-40 and compute_fbank.py:22-61: forward_stft with
+ * apply_abs (utils.py:130-135; cmat_abs, utils.py:30-42), then per flag, in this order,
+ *   SETK_FEAT_POW  the rounded magnitude squared               (np.power(., 2), utils.py:132-133)
+ *   SETK_FEAT_MEL  np.dot(mel, .) with the plan's mel table    (compute_fbank.py:49-51)
+ *   SETK_FEAT_LOG  log(max(., FLT_EPSILON))                    (utils.py:134-135, compute_fbank.py:52-53)
+ * sample_scale multiplies the magnitude before those steps: for a power of two this equals scaling
+ * the samples, bit for bit (x / 32768 with scale 32768 gives the features of the raw int16 values,
+ * read_wav(normalize=False), utils.py:65-92).
+ *   out  f32 [B][C][T][D], T = setk_num_frames(plan, N), D = setk_num_bins(plan), or num_mel under
+ *        SETK_FEAT_MEL; frames past an utterance's own count are zero rows.
+ * n_fft 512 (even hop) and 1024 (hop % 4 == 0) run fused from the audio: the STFT stays on chip.  Other
+ * geometries run the generic STFT into the plan's workspace, then the same tail.
+ * SETK_EINVAL: null plan / audio / out, SETK_FEAT_MEL without a table (setk_plan_set_mel), unknown
+ * flag bits, sample_scale not finite and > 0.  SETK_ESHAPE: the batch checks of setk_stft, B > 65535. */
+#define SETK_FEAT_POW 1u
+#define SETK_FEAT_MEL 2u
+#define SETK_FEAT_LOG 4u
+int setk_spectral_feats(setk_plan_t* plan, const float* audio, const int32_t* n_samples, int32_t B, int32_t N,
+                        uint32_t flags, float sample_scale, float* out, void* stream);
+
+/* The plan's mel filterbank for setk_spectral_feats: librosa.filters.mel(sr, n_fft, n_mels, fmin, fmax,
+ * htk=True) as compute_fbank.py:45-48 builds it (setk_b200.libs.filters.mel restates it on the host).
+ *   mel_host  f32 [num_mel][F] host matrix, F = setk_num_bins(plan): finite, >= 0.  Each row keeps the
+ *             bins from its first to its last non-zero weight (the exact zeros outside are skipped);
+ *             an all-zero row gives zero features.  num_mel = 0 clears the table.
+ * Synchronous (uploads like setk_plan_create's window).  SETK_EINVAL: null plan, mel_host null with
+ * num_mel > 0, num_mel outside [0, 1024], a negative or non-finite weight. */
+int setk_plan_set_mel(setk_plan_t* plan, int32_t num_mel, const float* mel_host);
 
 /* THE METRIC KERNEL.  Fused multichannel STFT + mask-weighted spatial
  * covariance: data_handler.py:502-503 -> beamformer.py:279-281 -> 87-103

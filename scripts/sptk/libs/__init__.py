@@ -12,7 +12,8 @@ _ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.dirname(os.path.
 if _ROOT not in sys.path:
     sys.path.insert(0, _ROOT)
 
-for _name in ("utils", "stft", "beamformer", "cluster", "wpe", "spatial", "data_handler", "opts", "sampler", "metric"):
+for _name in ("utils", "stft", "beamformer", "cluster", "wpe", "spatial", "data_handler", "opts", "sampler", "metric",
+              "filters", "exraw"):
     _mod = importlib.import_module("setk_b200.libs." + _name)
     sys.modules[__name__ + "." + _name] = _mod
     globals()[_name] = _mod

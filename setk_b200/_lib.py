@@ -10,7 +10,7 @@ package itself.)
 """
 import ctypes
 import os
-from ctypes import (POINTER, Structure, c_char_p, c_double, c_int, c_int32,
+from ctypes import (POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int32,
                     c_int64, c_uint32, c_void_p)
 
 import numpy as np
@@ -29,6 +29,8 @@ ST_ERROR_MASK = 31
 BF_MVDR, BF_MPDR, BF_MPDR_WHITEN, BF_GEVD, BF_PMWF, BF_PEVD = 0, 1, 2, 3, 4, 5
 RANK1_NONE, RANK1_EIG, RANK1_GEV = 0, 1, 2
 F_CLIP_MASK, F_MASK_FT = 1, 2
+FEAT_POW, FEAT_MEL, FEAT_LOG = 1, 2, 4
+FEAT_MAX_MEL = 1024
 C64, C128 = 0, 1
 SSL_ML, SSL_SRP, SSL_MUSIC = 0, 1, 2
 SSL_MAX_MASKS = 8
@@ -95,6 +97,9 @@ _PROTOTYPES = {
     "setk_stft_cov": (c_int, [c_void_p, c_void_p, c_void_p, c_int32, c_int32,
                               c_void_p, c_void_p, c_uint32, c_void_p, c_void_p,
                               c_void_p, c_void_p]),
+    "setk_spectral_feats": (c_int, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_uint32, c_float,
+                                    c_void_p, c_void_p]),
+    "setk_plan_set_mel": (c_int, [c_void_p, c_int32, c_void_p]),
     "setk_cov": (c_int, [c_void_p, c_void_p, c_uint32, c_int32, c_int32,
                          c_int32, c_int32, c_void_p, c_void_p]),
     "setk_weights": (c_int, [c_int32, c_double, c_int32, c_int32, c_int32,

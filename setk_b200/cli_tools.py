@@ -411,3 +411,198 @@ def steer_vector_main(argv=None):
     if args.normalize:
         sv = sv / sv.shape[-1]**0.5
     np.save(args.steer_vector, sv.transpose(0, 2, 1))       # A x M x F
+
+
+# ---------------------------------------------------------------------------------------------
+# compute_spectrogram.py (reference: run :19-40, flags :43-84) and compute_fbank.py (run :22-61,
+# flags :64-121): ragged device batches of channel 0.  A reader thread loads consecutive keys (raw
+# int16 for PCM-16 files); two pinned staging sets alternate, so that filling one overlaps the device
+# work and the copy back of the other; H2D, setk_pcm16_to_float, setk_spectral_feats, D2H; entries are
+# written in scp order.  The bytes written do not depend on --batch-size.
+# ---------------------------------------------------------------------------------------------
+_FEAT_FORMATS = ("kaldi", "exraw")
+_FEAT_FLAGS = [("--scp", str, "", None, "If assigned, generate corresponding scripts for archives"),
+               ("--format", str, "kaldi", None, "Output archive format (kaldi | exraw), see sptk/libs/exraw.py"),
+               ("--batch-size", int, 64, "batch_size", "utterances per device batch")]
+
+
+class _FeatStaging(object):
+    """One pinned host set: int16 or float32 input [B][N], lengths, features out [B][T][D], and its event."""
+
+    def __init__(self, batch, n_cap, t_cap, D, pcm16, pin):
+        self.pcm16 = pcm16
+        self.x = torch.zeros((batch, n_cap), dtype=torch.int16 if pcm16 else torch.float32, pin_memory=pin)
+        self.lens = torch.zeros((batch,), dtype=torch.int32, pin_memory=pin)
+        self.out = torch.empty((batch, t_cap, D), dtype=torch.float32, pin_memory=pin)
+        self.event = None
+        self.job = None
+
+
+def _feature_batches(reader, batch_size):
+    """Lists of (key, channel-0 samples) of consecutive keys, loaded by a background thread."""
+    import queue
+    import threading
+    q = queue.Queue(maxsize=4)
+    err = []
+
+    def load():
+        try:
+            batch = []
+            for key in reader.index_keys:
+                x = reader.read(key)
+                batch.append((key, np.ascontiguousarray(x[0] if x.ndim == 2 else x)))
+                if len(batch) == batch_size:
+                    q.put(batch)
+                    batch = []
+            if batch:
+                q.put(batch)
+        except BaseException as e:     # surfaced by the consumer
+            err.append(e)
+        finally:
+            q.put(None)
+
+    threading.Thread(target=load, daemon=True).start()
+    while True:
+        batch = q.get()
+        if batch is None:
+            break
+        yield batch
+    if err:
+        raise err[0]
+
+
+def _run_features(args, apply_log, apply_pow=False, mel_args=None, normalize=True):
+    """
+    Features of channel 0 of every utterance of args.wav_scp.  normalize=False feeds the raw sample
+    values (read_wav(normalize=False): int16 values of PCM-16, data >> 16 of 32-bit PCM, ...).  Every
+    utterance is staged as its normalised-domain samples v = raw / 32768 (PCM-16 on the device, other
+    formats on the host, exactly: a power of two) and setk_spectral_feats scales |X| back by 32768, so
+    an utterance gives the same bits whatever else shares its batch.
+    """
+    from . import plan as _plan
+    from .libs.exraw import BinaryWriter
+    from .libs.utils import default_device, get_plan
+    from .libs.data_handler import WaveReader
+    if args.format not in _FEAT_FORMATS:
+        raise SystemExit(f"--format: invalid choice {args.format!r}")
+    if args.batch_size < 1:
+        raise SystemExit("--batch-size must be >= 1")
+    dev = default_device()
+    reader = WaveReader(args.wav_scp, normalize=normalize, raw_pcm16=True)
+    sample_scale = 1.0 if normalize else 32768.0
+    writer_cls = ArchiveWriter if args.format == "kaldi" else BinaryWriter
+    D = mel_args["n_mels"] if mel_args else _bins(args)
+    weights = None
+    if mel_args:
+        from .libs.filters import mel
+        n_fft = nextpow2(args.frame_len) if args.round_power_of_two else args.frame_len
+        weights = mel(args.sr, n_fft, htk=True, **mel_args)
+    staging = [None, None]
+    mel_plan = [None]
+    done = [0]
+
+    def finish(writer, st):
+        st.event.synchronize()
+        for b, (key, T) in enumerate(st.job):
+            writer.write(key, st.out[b, :T].numpy().copy())
+            done[0] += 1
+        st.job = None
+
+    def host_samples(x):
+        """x in the normalised domain as float32 (exact: x / 32768 or x as read)."""
+        if x.dtype == np.int16 or not normalize:
+            return x.astype(np.float32) / np.float32(32768.0)
+        return x.astype(np.float32)
+
+    short = None     # the error of an utterance too short for one frame, raised once the keys before it are written
+    with writer_cls(args.dup_ark, args.scp) as writer:
+        try:
+            for i, batch in enumerate(_feature_batches(reader, args.batch_size)):
+                N = max(x.shape[-1] for _, x in batch)
+                pl = get_plan(1, args.frame_len, args.frame_hop, args.center, args.round_power_of_two, args.window,
+                              N, dev, batch=args.batch_size)
+                frames = []
+                for j, (_, x) in enumerate(batch):
+                    try:
+                        frames.append(pl.num_frames(x.shape[-1]))
+                    except ValueError as e:          # librosa's error on a too-short input stops the run
+                        short, batch = e, batch[:j]
+                        break
+                if batch:
+                    B = len(batch)
+                    N = max(x.shape[-1] for _, x in batch)
+                    T = pl.num_frames(N)
+                    pcm16 = all(x.dtype == np.int16 for _, x in batch)
+                    if weights is not None and mel_plan[0] is not pl:
+                        pl.set_mel(weights)
+                        mel_plan[0] = pl
+                    st = staging[i % 2]
+                    if st is not None and st.job is not None:
+                        finish(writer, st)
+                    if st is None or st.pcm16 != pcm16 or st.x.shape[1] < N or st.out.shape[1] < T:
+                        st = staging[i % 2] = _FeatStaging(args.batch_size, N, T, D, pcm16, dev.type == "cuda")
+                    xs = st.x[:B, :N]
+                    xs.zero_()
+                    for b, (_, x) in enumerate(batch):
+                        xs[b, :x.shape[-1]] = torch.from_numpy(x if pcm16 else host_samples(x))
+                        st.lens[b] = x.shape[-1]
+                    x_dev = xs.to(dev, non_blocking=True)
+                    audio = (_plan.pcm16_to_float(x_dev) if pcm16 else x_dev).view(B, 1, N)
+                    lens = st.lens[:B].to(dev, non_blocking=True)
+                    feats = pl.spectral_feats(audio, n_samples=lens, apply_pow=apply_pow, mel=weights is not None,
+                                              apply_log=apply_log, sample_scale=sample_scale)
+                    st.out[:B, :T].copy_(feats[:, 0], non_blocking=True)
+                    if dev.type == "cuda":
+                        st.event = torch.cuda.Event()
+                        st.event.record(torch.cuda.current_stream(dev))
+                    else:
+                        st.event = type("_Done", (), {"synchronize": staticmethod(lambda: None)})
+                    st.job = [(key, t) for (key, _), t in zip(batch, frames)]
+                    if done[0] and done[0] % 1000 < B:
+                        logger.info(f"Processed {done[0]} utterances...")
+                    prev = staging[(i + 1) % 2]
+                    if prev is not None and prev.job is not None:
+                        finish(writer, prev)
+                if short is not None:
+                    break
+        finally:    # the keys before a failure are written, as the reference's loop writes them
+            for st in staging:      # each batch finishes the one before it: at most one is pending here
+                if st is not None and st.job is not None:
+                    finish(writer, st)
+    if short is not None:
+        raise short
+    logger.info("Process {:d} utterances".format(done[0]))
+
+
+def spectrogram_main(argv=None):
+    args = _parser(
+        "Command to extract spectrogram features (magnitude, power or log, channel 0) on the GPU and write "
+        "them as Kaldi (or exraw) archives",
+        [("wav_scp", "Source location of wave scripts in kaldi format"),
+         ("dup_ark", "Location to dump spectrogram features")],
+        _FEAT_FLAGS + [
+            ("--apply-log", strtobool, False, None, "If true, using log spectrogram instead of linear"),
+            ("--apply-pow", strtobool, False, None, "If true, extract power spectrum instead of magnitude spectrum"),
+            # parsed and never passed on by the reference: samples are always int16 / 32768
+            ("--normalize-samples", strtobool, False, "normalize", "If true, normalize sample values between "
+             "[-1, 1] (accepted and ignored, as in the reference)")]).parse_args(argv)
+    _run_features(args, args.apply_log, apply_pow=args.apply_pow)
+
+
+def fbank_main(argv=None):
+    args = _parser(
+        "Command to extract mel-spectrogram/fbank features (channel 0) on the GPU and write them as Kaldi "
+        "(or exraw) archives",
+        [("wav_scp", "Source location of wave scripts in kaldi format"),
+         ("dup_ark", "Location to dump spectrogram's features")],
+        _FEAT_FLAGS + [
+            ("--sr", int, 16000, None, "Waveform data sample rate"),
+            ("--apply-log", strtobool, False, "log", "If true, using log mel-spectrogram instead of linear"),
+            ("--normalize-samples", strtobool, False, "norm", "If true, normalize sample values between [-1, 1]"),
+            ("--num-bins", int, 40, "num_bins", "Number of mel-bins defined in mel-filters"),
+            ("--min-freq", int, 0, "min_freq", "Low cutoff frequency for mel bins"),
+            ("--max-freq", int, 8000, "max_freq", "High cutoff frequency for mel bins")]).parse_args(argv)
+    if args.max_freq > args.sr // 2:
+        raise RuntimeError("Max frequency for mel exceeds sample frequency")
+    _run_features(args, args.log, mel_args=dict(n_mels=args.num_bins, fmin=args.min_freq, fmax=args.max_freq),
+                  normalize=args.norm)

@@ -182,6 +182,7 @@ int setk_plan_destroy(setk_plan_t* pl) {
   if (pl->d_cgmm_ws) cudaFree(pl->d_cgmm_ws);
   if (pl->d_peak) cudaFree(pl->d_peak);
   if (pl->d_tile_prefix) cudaFree(pl->d_tile_prefix);
+  if (pl->d_mel) cudaFree(pl->d_mel);
   free(pl);
   return SETK_OK;
 }
@@ -226,6 +227,69 @@ int setk_stft(setk_plan_t* pl, const float* audio, const int32_t* n_samples, int
     e = run_stft_generic(pl, audio, n_samples, B, N, T, static_cast<float2*>(stft_out), stream);
   }
   return done(e, "setk_stft");
+}
+
+int setk_plan_set_mel(setk_plan_t* pl, int32_t num_mel, const float* mel_host) {
+  if (!pl) return fail(SETK_EINVAL, "setk_plan_set_mel: null plan");
+  if (num_mel < 0 || num_mel > 1024) return fail(SETK_EINVAL, "setk_plan_set_mel: num_mel %d outside [0, 1024]", num_mel);
+  if (num_mel > 0 && !mel_host) return fail(SETK_EINVAL, "setk_plan_set_mel: null mel_host");
+  const int F = pl->geo.F;
+  // [num_mel][4] {first bin, bins, weight offset, 0}, then the weights of every band
+  std::vector<int> band(4 * (size_t)num_mel, 0);
+  std::vector<float> w;
+  for (int m = 0; m < num_mel; ++m) {
+    int lo = -1, hi = -1;
+    for (int k = 0; k < F; ++k) {
+      const float v = mel_host[(size_t)m * F + k];
+      if (!std::isfinite(v) || v < 0.f)
+        return fail(SETK_EINVAL, "setk_plan_set_mel: weight [%d][%d] = %g is not finite and >= 0", m, k, (double)v);
+      if (v > 0.f) { if (lo < 0) lo = k; hi = k; }
+    }
+    band[4 * m] = lo < 0 ? 0 : lo;
+    band[4 * m + 1] = lo < 0 ? 0 : hi - lo + 1;
+    band[4 * m + 2] = (int)w.size();
+    for (int k = lo; lo >= 0 && k <= hi; ++k) w.push_back(mel_host[(size_t)m * F + k]);
+  }
+  if (pl->d_mel) cudaFree(pl->d_mel);
+  pl->d_mel = nullptr; pl->num_mel = 0; pl->mel_weights = 0;
+  if (num_mel == 0) return SETK_OK;
+  const size_t band_bytes = sizeof(int) * band.size();
+  cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&pl->d_mel), band_bytes + sizeof(float) * w.size());
+  if (e == cudaSuccess) e = cudaMemcpy(pl->d_mel, band.data(), band_bytes, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && !w.empty())
+    e = cudaMemcpy(pl->d_mel + band.size(), w.data(), sizeof(float) * w.size(), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    if (pl->d_mel) cudaFree(pl->d_mel);
+    pl->d_mel = nullptr;
+    return cuda_fail(e, "setk_plan_set_mel");
+  }
+  pl->num_mel = num_mel;
+  pl->mel_weights = (int)w.size();
+  return SETK_OK;
+}
+
+int setk_spectral_feats(setk_plan_t* pl, const float* audio, const int32_t* n_samples, int32_t B, int32_t N,
+                        uint32_t flags, float sample_scale, float* out, void* stream) {
+  int rc = check_batch(pl, B, N, "setk_spectral_feats");
+  if (rc) return rc;
+  if (!audio || !out) return fail(SETK_EINVAL, "setk_spectral_feats: null buffer");
+  if (flags & ~(SETK_FEAT_POW | SETK_FEAT_MEL | SETK_FEAT_LOG))
+    return fail(SETK_EINVAL, "setk_spectral_feats: unknown flags 0x%x", flags);
+  if ((flags & SETK_FEAT_MEL) && !pl->d_mel)
+    return fail(SETK_EINVAL, "setk_spectral_feats: SETK_FEAT_MEL without a mel table (setk_plan_set_mel)");
+  if (!std::isfinite(sample_scale) || !(sample_scale > 0.f))
+    return fail(SETK_EINVAL, "setk_spectral_feats: sample_scale %g must be finite and > 0", (double)sample_scale);
+  if (B > 65535) return fail(SETK_ESHAPE, "setk_spectral_feats: batch %d > 65535", B);
+  const Geometry& g = pl->geo;
+  const int T = frames_of(N, g.n_fft, g.hop, g.pad);
+  if (feats_fused_supported(g))
+    return done(run_feats_fused(pl, audio, n_samples, B, N, T, flags, sample_scale, out, stream),
+                "setk_spectral_feats");
+  cudaError_t e = ensure(&pl->d_stft_ws, &pl->stft_ws_bytes, sizeof(float2) * (size_t)B * g.C * g.F * T);
+  if (e != cudaSuccess) return cuda_fail(e, "setk_spectral_feats(workspace)");
+  e = run_stft_generic(pl, audio, n_samples, B, N, T, pl->d_stft_ws, stream);
+  if (e == cudaSuccess) e = run_feats_stft(pl, pl->d_stft_ws, n_samples, B, N, T, flags, sample_scale, out, stream);
+  return done(e, "setk_spectral_feats");
 }
 
 int setk_cov(const void* stft, const float* mask, uint32_t flags, int32_t B, int32_t C, int32_t F,

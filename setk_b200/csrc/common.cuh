@@ -109,5 +109,6 @@ struct setk_plan {
   double* d_cgmm_ws;     size_t cgmm_ws_bytes;    // CGMM posteriors, partials, R^-1 (cgmm.cu)
   int* d_tile_prefix;   size_t tile_prefix_bytes;   // ragged batches: tiles before each utterance
   float* d_wave_ws;     size_t wave_ws_bytes;       // un-normalised wave of the PCM-16 output path
+  int* d_mel;           int num_mel, mel_weights;   // setk_plan_set_mel: [num_mel][4] bands, then the weights
   int sm_count;
 };

@@ -67,6 +67,13 @@ cudaError_t run_spill_to_bcft(const setk_plan* pl, const float2* xws, int B, int
 cudaError_t run_apply_spill(setk_plan* pl, const float2* xws, const void* w, int w_dtype, const float* post_mask,
                             int B, int T, float2* yws, void* stream);
 
+// ---- feats.cu: spectral features (magnitude / power / mel / log) ----
+bool feats_fused_supported(const Geometry& g);
+cudaError_t run_feats_fused(const setk_plan* pl, const float* audio, const int* n_samples, int B, int N, int T,
+                            unsigned flags, float scale, float* out, void* stream);
+cudaError_t run_feats_stft(const setk_plan* pl, const float2* stft, const int* n_samples, int B, int N, int T,
+                           unsigned flags, float scale, float* out, void* stream);
+
 // ---- cov_mma.cu: tensor-core covariance over the workspace (C >= 5) ----
 int cov_mma_bins_per_cta(int C);
 cudaError_t run_cov_mma(const CovSpillArgs& a, int B, void* stream);

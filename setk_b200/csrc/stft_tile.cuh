@@ -12,6 +12,7 @@
 //                half-size spectrum Z stays in shared memory
 //   split_bin  : X[k] (and X[256-k]) from Z[k], Z[256-k] with the bin's
 //                constant twiddle
+//   Tile1024, stage_tile1024 : the 1024-point tile of stft_spill.cu and feats.cu
 #pragma once
 #include "async_copy.cuh"
 #include "common.cuh"
@@ -224,6 +225,65 @@ __device__ __forceinline__ void split_pair(float2 zk, float2 zn, float2 tw, floa
   xk = f2add(e, p);
   const float2 m = f2sub(e, p);
   xm = make_float2(m.x, -m.y);
+}
+
+constexpr int kNfft2 = 1024;       // the second tile size (BASELINE config 3)
+constexpr int kBins2 = 513;
+
+// ---------------------------------------------------------------------------
+// n_fft = 1024 (513 bins): the same tile scheme with TT = 2 frames.  A
+// 1024-point real FFT is two 512-point real FFTs of the even and the odd
+// samples, i.e. two half-warp jobs  z_e[m] = x[4m] + i x[4m+2],
+// z_o[m] = x[4m+1] + i x[4m+3]  that share their (16-byte) shared-memory loads;
+//   X[k] = E[k] + W1024^k O[k],  E[k] = conj(E[512-k]) for k > 256.
+// ---------------------------------------------------------------------------
+template <int CG>
+struct Tile1024 {
+  static constexpr int TT = 2;
+  static constexpr int JOBS = TT * CG * 2;
+  int Lp; MBar* bar; float* win; float* audio0; float2* z;
+  SETK_HD static int staged_len(int hop) { return ((TT - 1) * hop + kNfft2 + 3) & ~3; }
+  SETK_HD static size_t floats(int hop) {
+    return 4 + (size_t)kNfft2 + 2 * (size_t)CG * staged_len(hop) + 2 * (size_t)JOBS * SETK_ZSLOT;
+  }
+  __device__ void carve(float* base, int hop) {
+    Lp = staged_len(hop);
+    bar = reinterpret_cast<MBar*>(base);
+    win = base + 4;
+    audio0 = win + kNfft2;
+    z = reinterpret_cast<float2*>(audio0 + 2 * CG * Lp);
+  }
+  __device__ float* abuf(int buf) const { return audio0 + buf * (CG * Lp); }
+};
+
+// all threads; true -> delivered by TMA on bar[buf]
+template <int CG>
+__device__ __forceinline__ bool stage_tile1024(const Tile1024<CG>& sm, int buf, const float* __restrict__ xb,
+                                               int N, int nb, int t0, int nt, int hop, int pad, bool vec_ok) {
+  const int p0 = t0 * hop;
+  const int need = (nt - 1) * hop + kNfft2;
+  const int i0 = p0 - pad;
+  float* dst = sm.abuf(buf);
+  if (vec_ok && i0 >= 0 && i0 + need <= nb) {
+    if (threadIdx.x == 0) {
+      fence_proxy_async();
+      mbar_expect_tx(&sm.bar[buf], (unsigned)(CG * need * sizeof(float)));
+#pragma unroll
+      for (int c = 0; c < CG; ++c)
+        bulk_g2s(dst + c * sm.Lp, xb + (long long)c * N + i0, (unsigned)(need * sizeof(float)),
+                 &sm.bar[buf]);
+    }
+    return true;
+  }
+#pragma unroll
+  for (int c = 0; c < CG; ++c) {
+    const float* src = xb + (long long)c * N;
+    for (int q = threadIdx.x; q < need; q += blockDim.x) {
+      const int i = pad ? reflect_index(p0 + q, pad, nb) : (p0 + q);
+      dst[c * sm.Lp + q] = src[i];
+    }
+  }
+  return false;
 }
 
 }  // namespace setk

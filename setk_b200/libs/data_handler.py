@@ -222,16 +222,25 @@ class SpectrogramReader(WaveReader):
         import torch
         from .utils import default_device
         opt = dict(self._defaults, **self.stft_kwargs)
-        for flag in ("apply_abs", "apply_log", "apply_pow"):
-            if opt.pop(flag, False):
-                raise NotImplementedError(f"SpectrogramReader: {flag} is not supported here")
+        apply_abs, apply_log, apply_pow = (opt.pop(f, False) for f in ("apply_abs", "apply_log", "apply_pow"))
+        if apply_log and not apply_abs:
+            warnings.warn("Ignore apply_abs=False because apply_log=True")
+            apply_abs = True
+        if apply_pow and not apply_abs:
+            raise NotImplementedError("SpectrogramReader: apply_pow of the complex STFT is not supported here")
         x = np.ascontiguousarray(np.atleast_2d(samps), dtype=np.float32)
         dev = default_device()
         plan = get_plan(x.shape[0], opt["frame_len"], opt["frame_hop"], opt["center"],
                         opt["round_power_of_two"], opt["window"], x.shape[1], dev)
-        spec = plan.stft(torch.from_numpy(x).to(dev)[None])[0]            # N x F x T
-        if opt["transpose"]:
-            spec = spec.transpose(-1, -2)
+        x = torch.from_numpy(x).to(dev)[None]
+        if apply_abs:       # forward_stft's abs / pow / log per channel (utils.py:130-135): N x T x F
+            spec = plan.spectral_feats(x, apply_pow=apply_pow, apply_log=apply_log)[0]
+            if not opt["transpose"]:
+                spec = spec.transpose(-1, -2)
+        else:
+            spec = plan.stft(x)[0]                                         # N x F x T
+            if opt["transpose"]:
+                spec = spec.transpose(-1, -2)
         if samps.ndim == 1:
             spec = spec[0]
         return spec if as_tensor else spec.cpu().numpy()

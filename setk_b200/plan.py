@@ -117,6 +117,7 @@ class StftPlan(object):
         self.center = bool(center)
         self.n_fft = nextpow2(frame_len) if round_power_of_two else int(frame_len)
         self.num_bins = self.n_fft // 2 + 1
+        self.num_mel = 0
         self.max_batch = int(max_batch)
         self.max_samples = int(max_samples)
         win = make_window(window, self.frame_len)
@@ -190,6 +191,51 @@ class StftPlan(object):
         _launch(self.device, "setk_stft_cov", self._h, _lib.ptr(audio), _lib.ptr(ns), B, N, _lib.ptr(mask_s),
                 _lib.ptr(mask_n), flags, _lib.ptr(Rs), _lib.ptr(Rn), _lib.ptr(maxabs))
         return Rs, Rn, maxabs
+
+    def set_mel(self, weights):
+        """
+        The mel filterbank of spectral_feats(mel=True): weights (M, F) float32 on the host, finite and
+        >= 0, 1 <= M <= 1024 (setk_b200.libs.filters.mel builds the reference's); None clears it.
+        """
+        if weights is None:
+            _lib.check(_lib.library().setk_plan_set_mel(self._h, 0, None))
+            self.num_mel = 0
+            return
+        if isinstance(weights, torch.Tensor):
+            weights = weights.detach().cpu().numpy()
+        w = np.ascontiguousarray(weights, dtype=np.float32)
+        if w.ndim != 2 or w.shape[1] != self.num_bins or not 1 <= w.shape[0] <= _lib.FEAT_MAX_MEL:
+            raise ValueError(f"mel weights must be (M, {self.num_bins}) with 1 <= M <= {_lib.FEAT_MAX_MEL}, "
+                             f"got {w.shape}")
+        if not (np.all(np.isfinite(w)) and np.all(w >= 0)):
+            raise ValueError("mel weights must be finite and >= 0")
+        with _ctx(self.device):
+            _lib.check(_lib.library().setk_plan_set_mel(self._h, w.shape[0], w.ctypes.data_as(ctypes.c_void_p)))
+        self.num_mel = w.shape[0]
+
+    def spectral_feats(self, audio, n_samples=None, apply_pow=False, mel=False, apply_log=False,
+                       sample_scale=1.0):
+        """
+        audio (B,C,N) -> (B,C,T,D) float32: |STFT| * sample_scale, then squared (apply_pow), projected
+        on the mel filters of set_mel (mel, D = M; else D = F) and log(max(., EPSILON)) (apply_log).
+        Frames past an utterance's n_samples are zero rows.
+        """
+        audio = self._check_audio(audio)
+        B, C, N = audio.shape
+        T = self.num_frames(N)
+        ns = _arg(n_samples, self.device, torch.int32, (B,), "n_samples")
+        if mel and not self.num_mel:
+            raise ValueError("spectral_feats(mel=True) needs set_mel() first")
+        scale = float(sample_scale)
+        if not (math.isfinite(scale) and scale > 0):
+            raise ValueError(f"sample_scale must be finite and > 0, got {sample_scale}")
+        D = self.num_mel if mel else self.num_bins
+        out = torch.empty((B, C, T, D), dtype=torch.float32, device=self.device)
+        flags = (_lib.FEAT_POW if apply_pow else 0) | (_lib.FEAT_MEL if mel else 0) | \
+            (_lib.FEAT_LOG if apply_log else 0)
+        _launch(self.device, "setk_spectral_feats", self._h, _lib.ptr(audio), _lib.ptr(ns), B, N, flags, scale,
+                _lib.ptr(out))
+        return out
 
     def cgmm_masks(self, audio, num_classes=2, num_iters=20, init_gamma=None, update_alpha=False,
                    n_samples=None):
