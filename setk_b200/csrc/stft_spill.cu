@@ -8,10 +8,10 @@
 // by one thread per (bin, matrix row).  Replaces the same reference code as
 // stft_cov_fused.cu (data_handler.py:492-503, beamformer.py:87-103,279-281).
 //
-//   stft_spill_kernel<CG,TT>  grid (chunks, channel groups of <= 4, B): the
-//       tile STFT of stft_tile.cuh (TMA-streamed audio, half-warp FFTs),
-//       split into X[k] and stored as  Xws[b][t][c][FP]  (c64, FP = 264:
-//       rows of bins are contiguous, 8-byte coalesced stores);  max|x|.
+//   stft_spill_kernel<CG,TT>, stft_spill1024_kernel<CG>  grid (chunks, channel
+//       groups of <= 4, B): the chunk driver tile_stft of stft_tile.cuh, whose
+//       X[k] are stored as  Xws[b][t][c][FP]  (c64, FP = 264 or 520: rows of
+//       bins are contiguous, 8-byte coalesced stores);  max|x|.
 //   cov_spill_kernel<C>       grid (chunks, C rows, B), thread per bin: row i
 //       accumulates  sum_t m x_i conj(x_j), j >= i  for (m_s, m_n) in fp32.
 //   cov_spill_finalize<C>     fixed-order sum over chunks, / max(sum m, 1e-6),
@@ -26,228 +26,55 @@
 
 namespace setk {
 
-constexpr int kSpillPitch = bin_pitch(kBins);
-constexpr int kSpillPitch2 = bin_pitch(kBins2);
-
-struct StftSpillArgs {
-  Geometry g;
-  const float* audio; const int* n_samples; int N;
-  int T;                 // frames of an N-sample utterance (workspace leading dim)
-  int frames_per_chunk, n_chunks;
-  const float* window;
-  float2* xws;           // [B][T][C][kSpillPitch]
+struct StftSpillArgs : TileChunkArgs {
+  float2* xws;           // [B][T][C][bin_pitch(F)]
   unsigned* maxabs_bits; // [B] or null
 };
+// moves a's audio and workspace on by c channels (launch_tile_chunks)
+static void shift_channels(StftSpillArgs& a, int c) {
+  a.audio += (long long)c * a.N;
+  a.xws += (long long)c * bin_pitch(a.g.F);
+}
 
-template <int CG, int TT>
-__global__ void __maxnreg__(96) stft_spill_kernel(StftSpillArgs a) {
+// Both spill kernels: the tile STFT of one chunk into the workspace, zeros for the frames past the
+// utterance's end, and max|x| into maxabs_bits.
+template <int CG, int TT, int NFFT>
+__device__ __forceinline__ void stft_spill_chunk(const StftSpillArgs& a) {
+  constexpr int F = NFFT / 2 + 1, P = bin_pitch(F);
   SETK_DYN_SMEM(float, smem);
   const int hop = a.g.hop, pad = a.g.pad, C = a.g.C;
-  TileSmem<CG, TT> sm;
+  TileSmem<CG, TT, NFFT> sm;
   sm.carve(smem, hop);
-  const int tid = threadIdx.x;
-  const int lane = tid & 31, warp = tid >> 5;
-  const int b = blockIdx.z, chunk = blockIdx.x, c0 = blockIdx.y * 4;
-  const int nb = a.n_samples ? a.n_samples[b] : a.N;
-  const int Tb = frames_of(nb, kNfft, hop, pad);
-  const int t_begin = chunk * a.frames_per_chunk;
-  const int t_end = imin(t_begin + a.frames_per_chunk, a.T);   // frames >= Tb are written as zeros
-
-  for (int n = tid; n < kNfft; n += blockDim.x) sm.win[n] = 0.5f * a.window[n];
-  if (tid == 0) { mbar_init(&sm.bar[0], 1); mbar_init(&sm.bar[1], 1); }
-  float w1s, w1c;
-  sincospif((float)(lane & 15) / 128.0f, &w1s, &w1c);
-  const float2 w1 = make_float2(w1c, -w1s);
-  const int bin = tid;
-  const bool bin_thread = bin < kBins;
-  const float2 tw = split_twiddle(bin);
-  const int zk = bin & (kM - 1), zn = (kM - bin) & (kM - 1);
+  const TileChunk ck = tile_chunk<NFFT>(a);
   float amax = 0.f;
-  const float* xb = a.audio + ((long long)b * C + c0) * a.N;
-  const bool vec_ok = ((a.N & 3) == 0) && ((hop & 3) == 0) && ((pad & 3) == 0) &&
-                      ((reinterpret_cast<uintptr_t>(a.audio) & 15) == 0);
-  const int t_live_end = imin(t_end, Tb);
-  unsigned par = 0;
-  bool async_cur = false;
-  if (t_begin < t_live_end)
-    async_cur = stage_tile_begin<CG, TT>(sm, 0, xb, a.N, nb, t_begin, imin(TT, t_live_end - t_begin),
-                                         hop, pad, vec_ok);
-  int buf = 0;
-  for (int t0 = t_begin; t0 < t_live_end; t0 += TT, buf ^= 1) {
-    const int nt = imin(TT, t_live_end - t0);
-    __syncthreads();
-    bool async_next = false;
-    if (t0 + TT < t_live_end)
-      async_next = stage_tile_begin<CG, TT>(sm, buf ^ 1, xb, a.N, nb, t0 + TT,
-                                            imin(TT, t_live_end - t0 - TT), hop, pad, vec_ok);
-    if (async_cur) {
-      mbar_wait(&sm.bar[buf], (par >> buf) & 1u);
-      par ^= 1u << buf;
-    }
-    if (warp < 8) fft_tile<CG, TT>(sm, buf, nt, hop, w1, amax);
-    async_cur = async_next;
-    __syncthreads();
-    if (bin_thread) {
-#pragma unroll
-      for (int j = 0; j < TT; ++j) {
-        if (j < nt) {
-#pragma unroll
-          for (int c = 0; c < CG; ++c) {
-            const float2* z = sm.z + (j * CG + c) * SETK_ZSLOT;
-            float2 x = split_bin(z[zk], z[zn], tw);
-            if (bin == 0 || bin == kM) x.y = 0.f;
-            a.xws[(((long long)b * a.T + (t0 + j)) * C + c0 + c) * kSpillPitch + bin] = x;
-          }
-        }
-      }
-    }
-  }
+  tile_stft(sm, a, ck, amax, [&](int t0, int j, int c, int k, float2 x) {
+    a.xws[(((long long)ck.b * a.T + (t0 + j)) * C + ck.c0 + c) * P + k] = x;
+  }, [](int, int) {});
   // frames past this utterance's own count (ragged batch): zeros
-  if (bin_thread) {
-    for (int t = imax(t_begin, t_live_end); t < t_end; ++t)
+  for (int t = imax(ck.t_begin, ck.t_live_end); t < ck.t_end; ++t)
 #pragma unroll
-      for (int c = 0; c < CG; ++c)
-        a.xws[(((long long)b * a.T + t) * C + c0 + c) * kSpillPitch + bin] = make_float2(0.f, 0.f);
-  }
+    for (int c = 0; c < CG; ++c)
+      for (int k = threadIdx.x; k < F; k += kChunkThreads)
+        a.xws[(((long long)ck.b * a.T + t) * C + ck.c0 + c) * P + k] = make_float2(0.f, 0.f);
   if (a.maxabs_bits) {
-    if (chunk == a.n_chunks - 1) {   // center=False tail that no frame covers
-      const int covered = (Tb > 0 ? (Tb - 1) * hop + kNfft - 2 * pad : 0);
+    if (blockIdx.x == gridDim.x - 1) {   // center=False tail that no frame covers
+      const int covered = (ck.Tb > 0 ? (ck.Tb - 1) * hop + NFFT - 2 * pad : 0);
+      const float* xb = ck.audio(a);
       for (int c = 0; c < CG; ++c)
-        for (int i = imax(covered, 0) + tid; i < nb; i += blockDim.x)
+        for (int i = imax(covered, 0) + threadIdx.x; i < ck.nb; i += blockDim.x)
           amax = fmaxf(amax, fabsf(xb[(long long)c * a.N + i]));
     }
     for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
-    if (lane == 0 && amax > 0.f) atomicMax(a.maxabs_bits + b, __float_as_uint(amax));
+    if ((threadIdx.x & 31) == 0 && amax > 0.f) atomicMax(a.maxabs_bits + ck.b, __float_as_uint(amax));
   }
 }
 
-template <int CG>
-__global__ void __launch_bounds__(288) stft_spill1024_kernel(StftSpillArgs a) {
-  SETK_DYN_SMEM(float, smem);
-  constexpr int TT = Tile1024<CG>::TT, JOBS = Tile1024<CG>::JOBS;
-  static_assert(JOBS <= 16, "one round of half-warp jobs");
-  const int hop = a.g.hop, pad = a.g.pad, C = a.g.C;   // hop % 4 == 0 (stft_spill_supported)
-  Tile1024<CG> sm;
-  sm.carve(smem, hop);
-  const int tid = threadIdx.x;
-  const int lane = tid & 31, warp = tid >> 5;
-  const int lane16 = lane & 15, half = lane >> 4;
-  const int b = blockIdx.z, chunk = blockIdx.x, c0 = blockIdx.y * 4;
-  const int nb = a.n_samples ? a.n_samples[b] : a.N;
-  const int Tb = frames_of(nb, kNfft2, hop, pad);
-  const int t_begin = chunk * a.frames_per_chunk;
-  const int t_end = imin(t_begin + a.frames_per_chunk, a.T);
+template <int CG, int TT>
+__global__ void __maxnreg__(96) stft_spill_kernel(StftSpillArgs a) { stft_spill_chunk<CG, TT, kNfft>(a); }
 
-  for (int n = tid; n < kNfft2; n += blockDim.x) sm.win[n] = 0.5f * a.window[n];
-  if (tid == 0) { mbar_init(&sm.bar[0], 1); mbar_init(&sm.bar[1], 1); }
-  float w1s, w1c;
-  sincospif((float)lane16 / 128.0f, &w1s, &w1c);
-  const float2 w1 = make_float2(w1c, -w1s);
-  // this thread's bins  k = tid, tid + 288  and their constants
-  int zk[2], zn[2];
-  float2 tw[2], wk[2];
-  bool cj[2];
-#pragma unroll
-  for (int s = 0; s < 2; ++s) {
-    const int k = tid + s * 288;
-    const int kk = k <= 256 ? k : 512 - k;           // bin of the 512-point halves
-    cj[s] = k > 256;
-    zk[s] = kk & (kM - 1); zn[s] = (kM - kk) & (kM - 1);
-    tw[s] = split_twiddle(kk);
-    float sn, cs;
-    sincospif((float)k / 512.0f, &sn, &cs);           // W1024^k
-    wk[s] = make_float2(cs, -sn);
-  }
-  float amax = 0.f;
-  const float* xb = a.audio + ((long long)b * C + c0) * a.N;
-  const bool vec_ok = ((a.N & 3) == 0) && ((pad & 3) == 0) &&
-                      ((reinterpret_cast<uintptr_t>(a.audio) & 15) == 0);
-  const int t_live_end = imin(t_end, Tb);
-  unsigned par = 0;
-  bool async_cur = false;
-  if (t_begin < t_live_end)
-    async_cur = stage_tile1024<CG>(sm, 0, xb, a.N, nb, t_begin, imin(TT, t_live_end - t_begin), hop, pad,
-                                   vec_ok);
-  int buf = 0;
-  for (int t0 = t_begin; t0 < t_live_end; t0 += TT, buf ^= 1) {
-    const int nt = imin(TT, t_live_end - t0);
-    __syncthreads();
-    bool async_next = false;
-    if (t0 + TT < t_live_end)
-      async_next = stage_tile1024<CG>(sm, buf ^ 1, xb, a.N, nb, t0 + TT, imin(TT, t_live_end - t0 - TT),
-                                      hop, pad, vec_ok);
-    if (async_cur) {
-      mbar_wait(&sm.bar[buf], (par >> buf) & 1u);
-      par ^= 1u << buf;
-    }
-    const int job = warp * 2 + half;                  // (frame, channel, parity)
-    if (job - half < JOBS) {                          // warp-uniform
-      const int fr = job / (2 * CG), rem = job - fr * 2 * CG;
-      const int ch = rem >> 1;                        // parity == half: both halves share the loads
-      float2 v[16];
-      const float* src = sm.abuf(buf) + ch * sm.Lp + fr * hop + 4 * lane16;
-      const float* wsrc = sm.win + 4 * lane16;
-      const bool live = fr < nt;
-#pragma unroll
-      for (int m1 = 0; m1 < 16; ++m1) {
-        float2 x = make_float2(0.f, 0.f);
-        if (live) {
-          const float4 s = *reinterpret_cast<const float4*>(src + 64 * m1);
-          const float4 w = *reinterpret_cast<const float4*>(wsrc + 64 * m1);
-          amax = fmaxf(amax, fmaxf(fmaxf(fabsf(s.x), fabsf(s.y)), fmaxf(fabsf(s.z), fabsf(s.w))));
-          x = half ? make_float2(s.y * w.y, s.w * w.w) : make_float2(s.x * w.x, s.z * w.z);
-        }
-        v[m1] = x;
-      }
-      float2* zs = sm.z + job * SETK_ZSLOT;
-      halfwarp_fft256(v, zs, lane16, w1);
-#pragma unroll
-      for (int s = 0; s < 16; ++s) zs[lane16 + 16 * kof(s)] = v[s];
-    }
-    async_cur = async_next;
-    __syncthreads();
-#pragma unroll
-    for (int s = 0; s < 2; ++s) {
-      const int k = tid + s * 288;
-      if (k < kBins2) {
-#pragma unroll
-        for (int j = 0; j < TT; ++j) {
-          if (j < nt) {
-#pragma unroll
-            for (int c = 0; c < CG; ++c) {
-              const float2* ze = sm.z + ((j * CG + c) * 2) * SETK_ZSLOT;
-              const float2* zo = ze + SETK_ZSLOT;
-              float2 e = split_bin(ze[zk[s]], ze[zn[s]], tw[s]);
-              float2 o = split_bin(zo[zk[s]], zo[zn[s]], tw[s]);
-              if (cj[s]) { e.y = -e.y; o.y = -o.y; }
-              float2 x = make_float2(e.x + wk[s].x * o.x - wk[s].y * o.y,
-                                     e.y + wk[s].x * o.y + wk[s].y * o.x);
-              if (k == 0 || k == kNfft2 / 2) x.y = 0.f;
-              a.xws[(((long long)b * a.T + (t0 + j)) * C + c0 + c) * kSpillPitch2 + k] = x;
-            }
-          }
-        }
-      }
-    }
-  }
-  for (int s = 0; s < 2; ++s) {
-    const int k = tid + s * 288;
-    if (k < kBins2)
-      for (int t = imax(t_begin, t_live_end); t < t_end; ++t)
-#pragma unroll
-        for (int c = 0; c < CG; ++c)
-          a.xws[(((long long)b * a.T + t) * C + c0 + c) * kSpillPitch2 + k] = make_float2(0.f, 0.f);
-  }
-  if (a.maxabs_bits) {
-    if (chunk == a.n_chunks - 1) {
-      const int covered = (Tb > 0 ? (Tb - 1) * hop + kNfft2 - 2 * pad : 0);
-      for (int c = 0; c < CG; ++c)
-        for (int i = imax(covered, 0) + tid; i < nb; i += blockDim.x)
-          amax = fmaxf(amax, fabsf(xb[(long long)c * a.N + i]));
-    }
-    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
-    if (lane == 0 && amax > 0.f) atomicMax(a.maxabs_bits + b, __float_as_uint(amax));
-  }
+template <int CG>
+__global__ void __launch_bounds__(kChunkThreads) stft_spill1024_kernel(StftSpillArgs a) {
+  stft_spill_chunk<CG, 2, kNfft2>(a);   // hop % 4 == 0 (stft_spill_supported)
 }
 
 // Beamformer.beamform on the workspace (beamformer.py:220-234, optional
@@ -419,50 +246,22 @@ size_t apply_spill_bytes(const Geometry& g, int B, int T) {
   return sizeof(float2) * (size_t)B * T * bin_pitch(g.F);
 }
 
-// channel groups [first_group, first_group + count) of CG channels each
-template <int CG>
-static cudaError_t run_spill_t(StftSpillArgs a, int B, void* stream, int first_group, int count) {
-  StftSpillArgs s = a;
-  s.audio = a.audio + (long long)first_group * 4 * a.N;      // the kernels take c0 from blockIdx.y
-  s.xws = a.xws + (long long)first_group * 4 * bin_pitch(a.g.F);
-  if (a.g.n_fft == kNfft2) {
-    const size_t smem = sizeof(float) * Tile1024<CG>::floats(a.g.hop);
-    cudaError_t e = cudaFuncSetAttribute(stft_spill1024_kernel<CG>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    return launch(stft_spill1024_kernel<CG>, dim3(a.n_chunks, count, B), dim3(288), smem, stream, false, s);
-  }
-  constexpr int TT = 4;
-  const size_t smem = sizeof(float) * TileSmem<CG, TT>::floats(a.g.hop);
-  cudaError_t e = cudaFuncSetAttribute(stft_spill_kernel<CG, TT>,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
-  return launch(stft_spill_kernel<CG, TT>, dim3(a.n_chunks, count, B), dim3(288), smem, stream, false, s);
-}
-
 cudaError_t run_stft_spill(setk_plan* pl, const float* audio, const int* n_samples, int B, int N, int T,
                            int n_chunks, float2* xws, unsigned* maxabs_bits, void* stream) {
-  const int TT = pl->geo.n_fft == kNfft2 ? 2 : 4;
   StftSpillArgs a;
   a.g = pl->geo;
   a.audio = audio; a.n_samples = n_samples; a.N = N; a.T = T;
-  a.n_chunks = n_chunks;
-  int fpc = (T + n_chunks - 1) / n_chunks;
-  a.frames_per_chunk = ((fpc + TT - 1) / TT) * TT;
   a.window = pl->d_window;
   a.xws = xws;
   a.maxabs_bits = maxabs_bits;
-  const int C = pl->geo.C;
-  const int full = C / 4, rem = C % 4;
-  cudaError_t e = cudaSuccess;
-  if (full > 0) e = run_spill_t<4>(a, B, stream, 0, full);
-  if (e != cudaSuccess) return e;
-  switch (rem) {
-    case 1: return run_spill_t<1>(a, B, stream, full, 1);
-    case 2: return run_spill_t<2>(a, B, stream, full, 1);
-    case 3: return run_spill_t<3>(a, B, stream, full, 1);
-    default: return e;
-  }
+  const int hop = a.g.hop;
+  const bool n1024 = a.g.n_fft == kNfft2;
+  return launch_tile_chunks(a, B, n_chunks, stream, [&](auto cg) {
+    constexpr int CG = decltype(cg)::value;
+    if (n1024)
+      return TileLaunch<StftSpillArgs>{stft_spill1024_kernel<CG>, sizeof(float) * TileSmem<CG, 2, kNfft2>::floats(hop)};
+    return TileLaunch<StftSpillArgs>{stft_spill_kernel<CG, 4>, sizeof(float) * TileSmem<CG, 4>::floats(hop)};
+  });
 }
 
 // C >= 5: the covariance is a real dense contraction (2C x 2C Gram blocks over T frames) and runs

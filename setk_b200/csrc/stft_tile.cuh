@@ -1,5 +1,6 @@
-// stft_tile.cuh -- the on-chip STFT of one tile of TT frames x C channels,
-// shared by the two fused kernels (stft_cov_fused.cu, apply_istft_fused.cu).
+// stft_tile.cuh -- the on-chip STFT of one tile of TT frames x C channels, shared by the fused
+// kernels (stft_cov_fused.cu, stft_cov_ws.cu, apply_istft_fused.cu) and the chunk-grid kernels
+// (stft_spill.cu, feats.cu).
 //
 //   stage_tile_begin : audio (global, f32 [C][N]) -> shared.  Interior tiles are
 //                streamed by TMA 1-D bulk copies (one elected thread, completion
@@ -12,17 +13,23 @@
 //                half-size spectrum Z stays in shared memory
 //   split_bin  : X[k] (and X[256-k]) from Z[k], Z[256-k] with the bin's
 //                constant twiddle
-//   Tile1024, stage_tile1024 : the 1024-point tile of stft_spill.cu and feats.cu
+//   fft_tile1024, bin1024 : the same for n_fft 1024 (TT = 2)
+//   tile_stft  : one CTA's chunk of frames of a chunk-grid launch, staged, transformed and handed
+//                to the caller's per-bin sink tile by tile; launch_tile_chunks launches such a
+//                kernel over every channel group of a batch
 #pragma once
 #include "async_copy.cuh"
 #include "common.cuh"
 #include "fft16.cuh"
+#include <type_traits>
 
 namespace setk {
 
 constexpr int kNfft = 512;      // frame size of the fused kernels
 constexpr int kM = 256;         // half-size complex transform
 constexpr int kBins = 257;
+constexpr int kNfft2 = 1024;    // the second tile size (BASELINE config 3)
+constexpr int kBins2 = 513;
 
 // ---------------------------------------------------------------------------
 // Balanced persistent schedule.  The work of a launch is the sequence of
@@ -71,43 +78,53 @@ SETK_HD inline int sched_grid(int total_max, int n_ctas, int min_quota) {
   return (total_max + q - 1) / q;
 }
 
-// Shared-memory carve-up common to both fused kernels.
-template <int C, int TT>
+// Shared-memory carve-up of a tile of NFFT-point frames.  An NFFT-point frame keeps NFFT / 512
+// half-size spectra Z (n_fft 1024: the even and the odd samples' 512-point transforms).
+template <int C, int TT, int NFFT = kNfft>
 struct TileSmem {
+  static constexpr int kZ = NFFT / kNfft;   // Z slots per (frame, channel)
   int Lp;            // staged samples per channel (padded to a multiple of 4)
   MBar* bar;         // [2] one per audio buffer
-  float* win;        // [512]  analysis window x 0.5
+  float* win;        // [NFFT]  analysis window x 0.5
   float* audio0;     // [2][C][Lp] double buffered (kept as base + offset so the
                      // compiler keeps shared-memory addressing, LDS not LD)
-  float2* z;         // [TT*C][SETK_ZSLOT]
-  SETK_HD static int staged_len(int hop) { return ((TT - 1) * hop + kNfft + 3) & ~3; }
+  float2* z;         // [TT*C*kZ][SETK_ZSLOT]
+  SETK_HD static int staged_len(int hop) { return ((TT - 1) * hop + NFFT + 3) & ~3; }
   SETK_HD static size_t floats(int hop) {
-    return 4 + (size_t)kNfft + 2 * (size_t)C * staged_len(hop) + 2 * (size_t)TT * C * SETK_ZSLOT;
+    return 4 + (size_t)NFFT + 2 * (size_t)C * staged_len(hop) + 2 * (size_t)TT * C * kZ * SETK_ZSLOT;
   }
   __device__ void carve(float* base, int hop) {
     Lp = staged_len(hop);
     bar = reinterpret_cast<MBar*>(base);
     win = base + 4;
-    audio0 = win + kNfft;
+    audio0 = win + NFFT;
     z = reinterpret_cast<float2*>(audio0 + 2 * C * Lp);
   }
   __device__ float* abuf(int buf) const { return audio0 + buf * (C * Lp); }
-  __device__ float* end() { return reinterpret_cast<float*>(z + TT * C * SETK_ZSLOT); }
+  __device__ float* end() { return reinterpret_cast<float*>(z + TT * C * kZ * SETK_ZSLOT); }
 };
+
+// True when frames [t0, t0+nt) of NFFT samples lie inside the signal and vec_ok allows 16-byte
+// copies: the tile is then delivered by TMA bulk copies, else element-wise.
+template <int NFFT = kNfft>
+__device__ __forceinline__ bool tile_bulk_ok(int t0, int nt, int hop, int pad, int nb, bool vec_ok) {
+  const int i0 = t0 * hop - pad;
+  return vec_ok && i0 >= 0 && i0 + (nt - 1) * hop + NFFT <= nb;
+}
 
 // Begin staging the samples of frames [t0, t0+nt) of every channel into
 // audio[buf].  Called by ALL threads (uniform).  Returns true when the tile is
 // delivered asynchronously (consumers must mbar_wait on bar[buf]); false when
 // it was written with ordinary stores (visible after the next __syncthreads).
-template <int C, int TT>
-__device__ __forceinline__ bool stage_tile_begin(const TileSmem<C, TT>& sm, int buf,
+template <int C, int TT, int NFFT>
+__device__ __forceinline__ bool stage_tile_begin(const TileSmem<C, TT, NFFT>& sm, int buf,
                                                  const float* __restrict__ xb, int N, int nb, int t0,
                                                  int nt, int hop, int pad, bool vec_ok) {
   const int p0 = t0 * hop;                      // first padded position of the tile
-  const int need = (nt - 1) * hop + kNfft;      // samples actually used
+  const int need = (nt - 1) * hop + NFFT;       // samples actually used
   const int i0 = p0 - pad;
   float* dst = sm.abuf(buf);
-  if (vec_ok && i0 >= 0 && i0 + need <= nb) {
+  if (tile_bulk_ok<NFFT>(t0, nt, hop, pad, nb, vec_ok)) {
     if (threadIdx.x == 0) {
       fence_proxy_async();
       mbar_expect_tx(&sm.bar[buf], (unsigned)(C * need * sizeof(float)));
@@ -127,43 +144,6 @@ __device__ __forceinline__ bool stage_tile_begin(const TileSmem<C, TT>& sm, int 
     }
   }
   return false;
-}
-
-// The same decision and the two delivery paths as separate pieces, for kernels
-// that give the bulk-copy issue to one producer warp.
-__device__ __forceinline__ bool tile_bulk_ok(int t0, int nt, int hop, int pad, int nb, bool vec_ok) {
-  const int i0 = t0 * hop - pad;
-  return vec_ok && i0 >= 0 && i0 + (nt - 1) * hop + kNfft <= nb;
-}
-template <int C, int TT>
-__device__ __forceinline__ void stage_tile_bulk(const TileSmem<C, TT>& sm, int buf,
-                                                const float* __restrict__ xb, int N, int t0, int nt,
-                                                int hop, int pad) {   // ONE thread
-  const int need = (nt - 1) * hop + kNfft;
-  const int i0 = t0 * hop - pad;
-  float* dst = sm.abuf(buf);
-  fence_proxy_async();
-  mbar_expect_tx(&sm.bar[buf], (unsigned)(C * need * sizeof(float)));
-#pragma unroll
-  for (int c = 0; c < C; ++c)
-    bulk_g2s(dst + c * sm.Lp, xb + (long long)c * N + i0, (unsigned)(need * sizeof(float)),
-             &sm.bar[buf]);
-}
-template <int C, int TT>
-__device__ __forceinline__ void stage_tile_scalar(const TileSmem<C, TT>& sm, int buf,
-                                                  const float* __restrict__ xb, int N, int nb, int t0,
-                                                  int nt, int hop, int pad) {   // ALL threads
-  const int p0 = t0 * hop;
-  const int need = (nt - 1) * hop + kNfft;
-  float* dst = sm.abuf(buf);
-#pragma unroll
-  for (int c = 0; c < C; ++c) {
-    const float* src = xb + (long long)c * N;
-    for (int q = threadIdx.x; q < need; q += blockDim.x) {
-      const int i = pad ? reflect_index(p0 + q, pad, nb) : (p0 + q);
-      dst[c * sm.Lp + q] = src[i];
-    }
-  }
 }
 
 // Forward FFT of every (frame, channel) of the tile by warps 0..NW-1, reading
@@ -227,9 +207,6 @@ __device__ __forceinline__ void split_pair(float2 zk, float2 zn, float2 tw, floa
   xm = make_float2(m.x, -m.y);
 }
 
-constexpr int kNfft2 = 1024;       // the second tile size (BASELINE config 3)
-constexpr int kBins2 = 513;
-
 // ---------------------------------------------------------------------------
 // n_fft = 1024 (513 bins): the same tile scheme with TT = 2 frames.  A
 // 1024-point real FFT is two 512-point real FFTs of the even and the odd
@@ -237,53 +214,216 @@ constexpr int kBins2 = 513;
 // z_o[m] = x[4m+1] + i x[4m+3]  that share their (16-byte) shared-memory loads;
 //   X[k] = E[k] + W1024^k O[k],  E[k] = conj(E[512-k]) for k > 256.
 // ---------------------------------------------------------------------------
+// Forward FFT of every (frame, channel) of a 1024-point tile: job = (frame, channel, parity) on one
+// half-warp, all jobs in one round of 288 threads.  A dead frame (fr >= nt) transforms zeros.
 template <int CG>
-struct Tile1024 {
-  static constexpr int TT = 2;
-  static constexpr int JOBS = TT * CG * 2;
-  int Lp; MBar* bar; float* win; float* audio0; float2* z;
-  SETK_HD static int staged_len(int hop) { return ((TT - 1) * hop + kNfft2 + 3) & ~3; }
-  SETK_HD static size_t floats(int hop) {
-    return 4 + (size_t)kNfft2 + 2 * (size_t)CG * staged_len(hop) + 2 * (size_t)JOBS * SETK_ZSLOT;
+__device__ __forceinline__ void fft_tile1024(const TileSmem<CG, 2, kNfft2>& sm, int buf, int nt, int hop,
+                                             float2 w1, float& amax) {
+  constexpr int JOBS = 2 * CG * 2;
+  static_assert(JOBS <= 16, "one round of half-warp jobs");
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int lane16 = lane & 15, half = lane >> 4;
+  const int job = warp * 2 + half;                  // (frame, channel, parity)
+  if (job - half < JOBS) {                          // warp-uniform
+    const int fr = job / (2 * CG), rem = job - fr * 2 * CG;
+    const int ch = rem >> 1;                        // parity == half: both halves share the loads
+    float2 v[16];
+    const float* src = sm.abuf(buf) + ch * sm.Lp + fr * hop + 4 * lane16;
+    const float* wsrc = sm.win + 4 * lane16;
+    const bool live = fr < nt;
+#pragma unroll
+    for (int m1 = 0; m1 < 16; ++m1) {
+      float2 x = make_float2(0.f, 0.f);
+      if (live) {
+        const float4 s = *reinterpret_cast<const float4*>(src + 64 * m1);
+        const float4 w = *reinterpret_cast<const float4*>(wsrc + 64 * m1);
+        amax = fmaxf(amax, fmaxf(fmaxf(fabsf(s.x), fabsf(s.y)), fmaxf(fabsf(s.z), fabsf(s.w))));
+        x = half ? make_float2(s.y * w.y, s.w * w.w) : make_float2(s.x * w.x, s.z * w.z);
+      }
+      v[m1] = x;
+    }
+    float2* zs = sm.z + job * SETK_ZSLOT;
+    halfwarp_fft256(v, zs, lane16, w1);
+#pragma unroll
+    for (int s = 0; s < 16; ++s) zs[lane16 + 16 * kof(s)] = v[s];
   }
-  __device__ void carve(float* base, int hop) {
-    Lp = staged_len(hop);
-    bar = reinterpret_cast<MBar*>(base);
-    win = base + 4;
-    audio0 = win + kNfft2;
-    z = reinterpret_cast<float2*>(audio0 + 2 * CG * Lp);
-  }
-  __device__ float* abuf(int buf) const { return audio0 + buf * (CG * Lp); }
+}
+
+// X[k] of a 1024-point tile from the even / odd half spectra ze, ze + SETK_ZSLOT of one (frame,
+// channel): zk, zn, tw are those of the 512-point bin kk = min(k, 512 - k), cj = k > 256, wk = W1024^k
+__device__ __forceinline__ float2 bin1024(const float2* ze, int k, int zk, int zn, float2 tw, bool cj,
+                                          float2 wk) {
+  const float2* zo = ze + SETK_ZSLOT;
+  float2 e = split_bin(ze[zk], ze[zn], tw);
+  float2 o = split_bin(zo[zk], zo[zn], tw);
+  if (cj) { e.y = -e.y; o.y = -o.y; }
+  float2 x = make_float2(e.x + wk.x * o.x - wk.y * o.y,
+                         e.y + wk.x * o.y + wk.y * o.x);
+  if (k == 0 || k == kNfft2 / 2) x.y = 0.f;
+  return x;
+}
+
+// ---------------------------------------------------------------------------
+// Chunk grid (stft_spill.cu, feats.cu): grid (chunks, channel groups, B) of kChunkThreads-thread
+// CTAs.  CTA (x, y, z) runs frames [x * frames_per_chunk, +frames_per_chunk) of the CG channels from
+// 4y (counted from the launch's first channel) of utterance z, with TT = 4 frames per tile at n_fft
+// 512 and 2 at 1024.
+// ---------------------------------------------------------------------------
+constexpr int kChunkThreads = 288;
+
+struct TileChunkArgs {
+  Geometry g;
+  const float* audio; const int* n_samples; int N;
+  int T;                 // frames of an N-sample utterance (rows of every output block)
+  int frames_per_chunk;  // a multiple of TT
+  const float* window;
 };
 
-// all threads; true -> delivered by TMA on bar[buf]
-template <int CG>
-__device__ __forceinline__ bool stage_tile1024(const Tile1024<CG>& sm, int buf, const float* __restrict__ xb,
-                                               int N, int nb, int t0, int nt, int hop, int pad, bool vec_ok) {
-  const int p0 = t0 * hop;
-  const int need = (nt - 1) * hop + kNfft2;
-  const int i0 = p0 - pad;
-  float* dst = sm.abuf(buf);
-  if (vec_ok && i0 >= 0 && i0 + need <= nb) {
-    if (threadIdx.x == 0) {
-      fence_proxy_async();
-      mbar_expect_tx(&sm.bar[buf], (unsigned)(CG * need * sizeof(float)));
-#pragma unroll
-      for (int c = 0; c < CG; ++c)
-        bulk_g2s(dst + c * sm.Lp, xb + (long long)c * N + i0, (unsigned)(need * sizeof(float)),
-                 &sm.bar[buf]);
-    }
-    return true;
+struct TileChunk {       // one CTA's share of a chunk-grid launch
+  int b, c0;             // utterance, first channel of the group
+  int nb, Tb;            // the utterance's samples and frames
+  int t_begin, t_end;    // the chunk's frames
+  int t_live_end;        // min(t_end, Tb): frames [t_live_end, t_end) are past the utterance's end
+  __device__ const float* audio(const TileChunkArgs& a) const {   // channel c0 of utterance b
+    return a.audio + ((long long)b * a.g.C + c0) * a.N;
   }
+};
+
+// this CTA's chunk
+template <int NFFT>
+__device__ __forceinline__ TileChunk tile_chunk(const TileChunkArgs& a) {
+  TileChunk ck;
+  ck.b = blockIdx.z;
+  ck.c0 = blockIdx.y * 4;
+  ck.nb = a.n_samples ? a.n_samples[ck.b] : a.N;
+  ck.Tb = frames_of(ck.nb, NFFT, a.g.hop, a.g.pad);
+  ck.t_begin = blockIdx.x * a.frames_per_chunk;
+  ck.t_end = imin(ck.t_begin + a.frames_per_chunk, a.T);
+  ck.t_live_end = imin(ck.t_end, ck.Tb);
+  return ck;
+}
+
+// All threads: the tile STFT of chunk ck, two audio buffers deep (the next tile is staged while this
+// one is transformed).  For every tile of frames [t0, t0 + nt), bin(t0, j, c, k, X) runs for each
+// live frame t0 + j, channel c0 + c and bin k = threadIdx.x + 288 s of this thread, then tile(t0, nt)
+// runs on all threads.  amax gathers max |sample| of the frames read.
+template <int CG, int TT, int NFFT, class Bin, class Tile>
+__device__ __forceinline__ void tile_stft(const TileSmem<CG, TT, NFFT>& sm, const TileChunkArgs& a,
+                                          const TileChunk& ck, float& amax, Bin bin, Tile tile) {
+  constexpr int S = NFFT / kNfft;                       // bins per thread
+  const int hop = a.g.hop, pad = a.g.pad;
+  const int tid = threadIdx.x;
+  for (int n = tid; n < NFFT; n += blockDim.x) sm.win[n] = 0.5f * a.window[n];
+  if (tid == 0) { mbar_init(&sm.bar[0], 1); mbar_init(&sm.bar[1], 1); }
+  float w1s, w1c;
+  sincospif((float)(tid & 15) / 128.0f, &w1s, &w1c);
+  const float2 w1 = make_float2(w1c, -w1s);
+  // the split constants of this thread's bins: those of the 512-point bin kk, and at n_fft 1024
+  // the fold cj = k > 256 and the twiddle wk = W1024^k
+  int zk[S], zn[S];
+  float2 tw[S], wk[S];
+  bool cj[S];
 #pragma unroll
-  for (int c = 0; c < CG; ++c) {
-    const float* src = xb + (long long)c * N;
-    for (int q = threadIdx.x; q < need; q += blockDim.x) {
-      const int i = pad ? reflect_index(p0 + q, pad, nb) : (p0 + q);
-      dst[c * sm.Lp + q] = src[i];
+  for (int s = 0; s < S; ++s) {
+    const int k = tid + s * kChunkThreads;
+    const int kk = (S == 1 || k <= kM) ? k : kNfft - k;
+    zk[s] = kk & (kM - 1); zn[s] = (kM - kk) & (kM - 1);
+    tw[s] = split_twiddle(kk);
+    if constexpr (S == 2) {
+      cj[s] = k > kM;
+      float sn, cs;
+      sincospif((float)k / 512.0f, &sn, &cs);
+      wk[s] = make_float2(cs, -sn);
     }
   }
-  return false;
+  const float* xb = ck.audio(a);
+  const bool vec_ok = ((a.N & 3) == 0) && ((hop & 3) == 0) && ((pad & 3) == 0) &&
+                      ((reinterpret_cast<uintptr_t>(a.audio) & 15) == 0);
+  unsigned par = 0;
+  bool async_cur = false;
+  if (ck.t_begin < ck.t_live_end)
+    async_cur = stage_tile_begin(sm, 0, xb, a.N, ck.nb, ck.t_begin, imin(TT, ck.t_live_end - ck.t_begin),
+                                 hop, pad, vec_ok);
+  int buf = 0;
+  for (int t0 = ck.t_begin; t0 < ck.t_live_end; t0 += TT, buf ^= 1) {
+    const int nt = imin(TT, ck.t_live_end - t0);
+    __syncthreads();
+    bool async_next = false;
+    if (t0 + TT < ck.t_live_end)
+      async_next = stage_tile_begin(sm, buf ^ 1, xb, a.N, ck.nb, t0 + TT, imin(TT, ck.t_live_end - t0 - TT),
+                                    hop, pad, vec_ok);
+    if (async_cur) {
+      mbar_wait(&sm.bar[buf], (par >> buf) & 1u);
+      par ^= 1u << buf;
+    }
+    if constexpr (S == 1) {
+      if (tid < 256) fft_tile<CG, TT>(sm, buf, nt, hop, w1, amax);   // warps 0..7
+    } else {
+      fft_tile1024<CG>(sm, buf, nt, hop, w1, amax);
+    }
+    async_cur = async_next;
+    __syncthreads();
+#pragma unroll
+    for (int s = 0; s < S; ++s) {
+      const int k = tid + s * kChunkThreads;
+      if (k < NFFT / 2 + 1) {
+#pragma unroll
+        for (int j = 0; j < TT; ++j) {
+          if (j < nt) {
+#pragma unroll
+            for (int c = 0; c < CG; ++c) {
+              const float2* z = sm.z + (j * CG + c) * S * SETK_ZSLOT;
+              float2 x;
+              if constexpr (S == 1) {
+                x = split_bin(z[zk[s]], z[zn[s]], tw[s]);
+                if (k == 0 || k == kM) x.y = 0.f;
+              } else {
+                x = bin1024(z, k, zk[s], zn[s], tw[s], cj[s], wk[s]);
+              }
+              bin(t0, j, c, k, x);
+            }
+          }
+        }
+      }
+    }
+    tile(t0, nt);
+  }
+}
+
+// Host: a chunk-grid kernel and its dynamic shared memory
+template <class Args>
+struct TileLaunch {
+  void (*kernel)(Args);
+  size_t smem;
+};
+
+// Host: runs a chunk-grid kernel over B utterances in n_chunks chunks of frames: one launch for the
+// C / 4 groups of 4 channels, one for the group of the C % 4 left, whose arguments are moved on to
+// its first channel by shift_channels(Args&, c).  pick(cg) gives the TileLaunch for groups of cg
+// channels (cg a std::integral_constant).
+template <class Args, class Pick>
+cudaError_t launch_tile_chunks(Args a, int B, int n_chunks, void* stream, Pick pick) {
+  const int TT = a.g.n_fft == kNfft2 ? 2 : 4;
+  const int fpc = (a.T + n_chunks - 1) / n_chunks;
+  a.frames_per_chunk = ((fpc + TT - 1) / TT) * TT;
+  auto run = [&](auto cg, int group0, int groups) -> cudaError_t {
+    const TileLaunch<Args> l = pick(cg);
+    cudaError_t e = cudaFuncSetAttribute(l.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l.smem);
+    if (e != cudaSuccess) return e;
+    Args s = a;
+    shift_channels(s, 4 * group0);
+    return launch(l.kernel, dim3(n_chunks, groups, B), dim3(kChunkThreads), l.smem, stream, false, s);
+  };
+  const int full = a.g.C / 4;
+  cudaError_t e = cudaSuccess;
+  if (full > 0) e = run(std::integral_constant<int, 4>(), 0, full);
+  if (e != cudaSuccess) return e;
+  switch (a.g.C % 4) {
+    case 1: return run(std::integral_constant<int, 1>(), full, 1);
+    case 2: return run(std::integral_constant<int, 2>(), full, 1);
+    case 3: return run(std::integral_constant<int, 3>(), full, 1);
+    default: return e;
+  }
 }
 
 }  // namespace setk
