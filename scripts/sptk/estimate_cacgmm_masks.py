@@ -24,7 +24,6 @@ Notes against the reference:
 import argparse
 import os
 import sys
-from pathlib import Path
 
 import numpy as np
 
@@ -35,32 +34,18 @@ if _ROOT not in sys.path:
 
 import torch  # noqa: E402
 
+from setk_b200 import cgmm_cli  # noqa: E402
 from setk_b200 import plan as _plan  # noqa: E402
-from setk_b200.libs.data_handler import NumpyReader, NumpyWriter, ScriptReader, WaveReader  # noqa: E402
 from setk_b200.libs.opts import StftParser, strtobool  # noqa: E402
-from setk_b200.libs.utils import default_device, forward_stft, get_logger, get_plan, nextpow2  # noqa: E402
+from setk_b200.libs.utils import get_logger  # noqa: E402
 
 logger = get_logger(__name__)
 
 
 def train_utterance(samps, args, init_mask, dev):
-    """samps C x N float32 -> (masks K x T x F float32 numpy, converged)."""
-    C, N = samps.shape
-    n_fft = nextpow2(args.frame_len) if args.round_power_of_two else args.frame_len
-    K, F = args.num_classes, n_fft // 2 + 1
-    tile = n_fft in (512, 1024) and args.frame_hop % 4 == 0 and args.frame_hop <= n_fft
-    audio = torch.from_numpy(np.ascontiguousarray(samps)).to(dev)[None]
-    if tile:
-        plan = get_plan(C, args.frame_len, args.frame_hop, bool(args.center), bool(args.round_power_of_two),
-                        args.window, N, dev)
-        T = plan.num_frames(N)
-    else:
-        stft = torch.stack([
-            forward_stft(audio[0, c], frame_len=args.frame_len, frame_hop=args.frame_hop,
-                         round_power_of_two=bool(args.round_power_of_two), center=bool(args.center),
-                         window=args.window, transpose=False) for c in range(C)
-        ])                                                                          # C x F x T
-        T = stft.shape[-1]
+    """samps C x N float32 -> masks K x T x F float32 numpy."""
+    K = args.num_classes
+    audio, plan, stft, T, F = cgmm_cli.observe(samps, args, dev)
     permu = None
     if args.solve_permu:
         if F not in _plan.PERMU_PLANS:
@@ -80,42 +65,15 @@ def train_utterance(samps, args, init_mask, dev):
     if init is not None:
         init = torch.from_numpy(np.ascontiguousarray(init))[None].to(dev)
     kw = dict(init_gamma=init, cgmm_init=cgmm_init, update_alpha=bool(args.update_alpha), permu_plan=permu)
-    if tile:
+    if plan is not None:
         masks, status = plan.cacgmm_masks(audio, K, args.num_iters, **kw)
     else:
         masks, status = _plan.cacgmm_from_stft(stft[None], K, args.num_iters, **kw)
     if permu is not None:
         logger.info("Permutation alignment done on each frequency")
-    return masks[0].cpu().numpy(), int(status.abs().sum()) == 0
-
-
-def run(args):
-    np.random.seed(args.seed)
-    dev = default_device()
-    wave_reader = WaveReader(args.wav_scp, sr=16000)
-    MaskReader = {"numpy": NumpyReader, "kaldi": ScriptReader}
-    init_mask_reader = MaskReader[args.fmt](args.init_mask) if args.init_mask else None
-
-    num_done = 0
-    with NumpyWriter(args.dst_dir) as writer:
-        dst_dir = Path(args.dst_dir)
-        for key, samps in wave_reader:
-            if (dst_dir / f"{key}.npy").exists():
-                logger.info(f"Training utterance {key} ... Skip")
-                continue
-            if samps.ndim == 1:
-                samps = samps[None]
-            init_mask = None
-            if init_mask_reader and key in init_mask_reader:
-                init_mask = init_mask_reader[key]          # K x T x F
-            masks, ok = train_utterance(np.asarray(samps, dtype=np.float32), args, init_mask, dev)
-            if not ok:
-                logger.warning(f"Training utterance {key} ... Failed")
-                continue
-            num_done += 1
-            writer.write(key, masks.astype(np.float32))
-            logger.info(f"Training utterance {key} ... Done")
-    logger.info(f"Train {num_done:d} utterances over {len(wave_reader):d}")
+    if int(status.abs().sum()) != 0:
+        raise cgmm_cli.Failed()
+    return masks[0].cpu().numpy()
 
 
 if __name__ == "__main__":
@@ -140,4 +98,4 @@ if __name__ == "__main__":
     parser.add_argument("--mask-format", type=str, dest="fmt", default="numpy", choices=["kaldi", "numpy"],
                         help="Mask storage format")
     args = parser.parse_args()
-    run(args)
+    cgmm_cli.run(args, train_utterance)

@@ -21,7 +21,6 @@ Notes against the reference:
 import argparse
 import os
 import sys
-from pathlib import Path
 
 import numpy as np
 
@@ -32,88 +31,47 @@ if _ROOT not in sys.path:
 
 import torch  # noqa: E402
 
+from setk_b200 import cgmm_cli  # noqa: E402
 from setk_b200.libs.cluster import CgmmTrainer, permu_aligner  # noqa: E402
-from setk_b200.libs.data_handler import (NumpyReader, NumpyWriter, ScriptReader,  # noqa: E402
-                                         WaveReader)
 from setk_b200.libs.opts import StftParser, strtobool  # noqa: E402
-from setk_b200.libs.utils import default_device, forward_stft, get_logger, get_plan, nextpow2  # noqa: E402
+from setk_b200.libs.utils import get_logger  # noqa: E402
 
 logger = get_logger(__name__)
 
 
 def train_utterance(samps, args, init_mask, dev):
-    """samps C x N float32 -> masks K x T x F float32 (numpy)."""
-    C, N = samps.shape
-    n_fft = nextpow2(args.frame_len) if args.round_power_of_two else args.frame_len
+    """samps C x N float32 -> the masks to write: K x T x F float32 numpy, T x F for two classes."""
     K = args.num_classes
-    audio = torch.from_numpy(np.ascontiguousarray(samps)).to(dev)[None]
-    init = None
-    if init_mask is not None:
-        g = torch.from_numpy(np.asarray(init_mask, dtype=np.float32)).to(dev)     # T x F or K x T x F
-        if g.dim() == 2:
-            g = torch.stack([g, 1 - g])                                            # cluster.py:428-429
-        init = g[None].contiguous()
-    if n_fft in (512, 1024) and args.frame_hop % 4 == 0 and args.frame_hop <= n_fft:
-        plan = get_plan(C, args.frame_len, args.frame_hop, bool(args.center),
-                        bool(args.round_power_of_two), args.window, N, dev)
-        if init is None and K != 2:
-            T, F = plan.num_frames(N), plan.num_bins
+    try:
+        if init_mask is not None:
+            logger.info("Using external TF-mask to initialize cgmm")
+        audio, plan, stft, T, F = cgmm_cli.observe(samps, args, dev)
+        init = None                                                                # K x T x F
+        if init_mask is not None:
+            init = torch.from_numpy(np.asarray(init_mask, dtype=np.float32)).to(dev)   # T x F or K x T x F
+            if init.dim() == 2:
+                init = torch.stack([init, 1 - init])                               # cluster.py:428-429
+        elif K != 2:
             g = np.random.uniform(size=[K, F, T])                                  # cluster.py:432-434
             g = g / np.sum(g, 0, keepdims=True)
-            init = torch.from_numpy(np.transpose(g, (0, 2, 1)).astype(np.float32)).to(dev)[None].contiguous()
-        masks, status = plan.cgmm_masks(audio, K, args.num_iters, init_gamma=init,
-                                        update_alpha=bool(args.update_alpha))
-        if int(status.abs().sum()) != 0:
-            raise RuntimeError("eigen-iteration did not converge")
-        return masks[0].cpu().numpy()
-    stft = torch.stack([
-        forward_stft(audio[0, c], frame_len=args.frame_len, frame_hop=args.frame_hop,
-                     round_power_of_two=bool(args.round_power_of_two), center=bool(args.center),
-                     window=args.window, transpose=False) for c in range(C)
-    ])                                                                             # C x F x T
-    gamma = None
-    if init is not None:
-        gamma = init[0].transpose(-1, -2)
-    elif K != 2:
-        g = np.random.uniform(size=[K, stft.shape[1], stft.shape[2]])
-        gamma = torch.from_numpy((g / np.sum(g, 0, keepdims=True)).astype(np.float32))
-    trainer = CgmmTrainer(stft, K, gamma=gamma, update_alpha=bool(args.update_alpha))
-    return trainer.train(args.num_iters).transpose(-1, -2).cpu().numpy()
-
-
-def run(args):
-    np.random.seed(args.seed)
-    dev = default_device()
-    wave_reader = WaveReader(args.wav_scp, sr=16000)
-    MaskReader = {"numpy": NumpyReader, "kaldi": ScriptReader}
-    init_mask_reader = MaskReader[args.fmt](args.init_mask) if args.init_mask else None
-
-    num_done = 0
-    with NumpyWriter(args.dst_dir) as writer:
-        dst_dir = Path(args.dst_dir)
-        for key, samps in wave_reader:
-            if (dst_dir / f"{key}.npy").exists():
-                logger.info(f"Training utterance {key} ... Skip")
-                continue
-            if samps.ndim == 1:
-                samps = samps[None]
-            init_mask = None
-            if init_mask_reader and key in init_mask_reader:
-                init_mask = init_mask_reader[key]          # T x F (or K x T x F)
-                logger.info("Using external TF-mask to initialize cgmm")
-            try:
-                masks = train_utterance(np.asarray(samps, dtype=np.float32), args, init_mask, dev)
-                num_done += 1
-                if args.solve_permu:
-                    masks = permu_aligner(masks)
-                    logger.info("Permutation alignment done on each frequency")
-                if args.num_classes == 2:
-                    masks = masks[0]
-                writer.write(key, masks.astype(np.float32))
-                logger.info(f"Training utterance {key} ... Done")
-            except RuntimeError as err:
-                logger.warning(f"Training utterance {key} ... Failed ({err})")
-    logger.info(f"Train {num_done:d} utterances over {len(wave_reader):d}")
+            init = torch.from_numpy(np.transpose(g, (0, 2, 1)).astype(np.float32)).to(dev)
+        if plan is not None:
+            masks, status = plan.cgmm_masks(audio, K, args.num_iters,
+                                            init_gamma=None if init is None else init[None].contiguous(),
+                                            update_alpha=bool(args.update_alpha))
+            if int(status.abs().sum()) != 0:
+                raise RuntimeError("eigen-iteration did not converge")
+            masks = masks[0].cpu().numpy()
+        else:
+            trainer = CgmmTrainer(stft, K, gamma=None if init is None else init.transpose(-1, -2),
+                                  update_alpha=bool(args.update_alpha))
+            masks = trainer.train(args.num_iters).transpose(-1, -2).cpu().numpy()
+        if args.solve_permu:
+            masks = permu_aligner(masks)
+            logger.info("Permutation alignment done on each frequency")
+    except RuntimeError as err:
+        raise cgmm_cli.Failed(err) from err
+    return masks[0] if K == 2 else masks
 
 
 if __name__ == "__main__":
@@ -138,4 +96,4 @@ if __name__ == "__main__":
     parser.add_argument("--mask-format", type=str, dest="fmt", default="numpy",
                         choices=["kaldi", "numpy"], help="Mask storage format")
     args = parser.parse_args()
-    run(args)
+    cgmm_cli.run(args, train_utterance)

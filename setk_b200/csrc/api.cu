@@ -510,62 +510,6 @@ int setk_apply_istft_pcm16(setk_plan_t* pl, const float* audio, const int32_t* n
                           stream);
 }
 
-int setk_cgmm_masks(setk_plan_t* pl, const float* audio, const int32_t* n_samples, int32_t B, int32_t N,
-                    int32_t num_classes, int32_t num_iters, const float* init_gamma, int32_t update_alpha,
-                    float* masks, uint32_t* status, void* stream) {
-  int rc = check_batch(pl, B, N, "setk_cgmm_masks");
-  if (rc) return rc;
-  if (!audio || !masks) return fail(SETK_EINVAL, "setk_cgmm_masks: null buffer");
-  if (num_classes < 2 || num_classes > 4)
-    return fail(SETK_EINVAL, "setk_cgmm_masks: num_classes %d outside 2..4", num_classes);
-  if (!init_gamma && num_classes != 2)
-    return fail(SETK_EINVAL, "setk_cgmm_masks: %d classes need init_gamma (the reference's start is random)",
-                num_classes);
-  if (num_iters < 0) return fail(SETK_EINVAL, "setk_cgmm_masks: num_iters %d", num_iters);
-  const Geometry& g = pl->geo;
-  if (!stft_spill_supported(g))
-    return fail(SETK_EUNSUPPORTED, "setk_cgmm_masks: needs n_fft 512 or 1024 (got %d, hop %d)", g.n_fft, g.hop);
-  const int T = frames_of(N, g.n_fft, g.hop, g.pad);
-  if (T < 1) return fail(SETK_ESHAPE, "setk_cgmm_masks: no frame in %d samples", N);
-  const int P = bin_pitch(g.F);
-  CgCtx ctx;
-  ctx.geo = g; ctx.sm_count = pl->sm_count;
-  cudaError_t e = ensure(&pl->d_cgmm_ws, &pl->cgmm_ws_bytes, cgmm_workspace_bytes(&ctx, B, T, num_classes, P));
-  if (e != cudaSuccess) return cuda_fail(e, "setk_cgmm_masks(workspace)");
-  rc = stft_to_bin_major(pl, audio, n_samples, B, N, T, nullptr, stream, "setk_cgmm_masks(workspace)",
-                         "setk_cgmm_masks");
-  if (rc) return rc;
-  e = run_cgmm(&ctx, pl->d_stft_ws, P, pl->d_cgmm_ws, n_samples, B, N, T, num_classes, num_iters, init_gamma,
-               update_alpha, masks, status, stream);
-  return done(e, "setk_cgmm_masks");
-}
-
-int setk_cgmm_stft(const void* stft, int32_t B, int32_t C, int32_t F, int32_t T, int32_t num_classes,
-                   int32_t num_iters, const float* init_gamma, int32_t update_alpha, float* masks,
-                   uint32_t* status, void* stream) {
-  if (!stft || !masks) return fail(SETK_EINVAL, "setk_cgmm_stft: null buffer");
-  if (B < 1 || B > 65535 || F < 1 || T < 1 || C < 1 || C > SETK_MAX_CHANNELS)
-    return fail(SETK_ESHAPE, "setk_cgmm_stft: bad shape B=%d C=%d F=%d T=%d", B, C, F, T);
-  if (num_classes < 2 || num_classes > 4)
-    return fail(SETK_EINVAL, "setk_cgmm_stft: num_classes %d outside 2..4", num_classes);
-  if (!init_gamma && num_classes != 2)
-    return fail(SETK_EINVAL, "setk_cgmm_stft: %d classes need init_gamma (the reference's start is random)",
-                num_classes);
-  if (num_iters < 0) return fail(SETK_EINVAL, "setk_cgmm_stft: num_iters %d", num_iters);
-  CgCtx ctx;
-  // frames are given, not derived from samples: a geometry whose frame count never limits
-  ctx.geo.C = C; ctx.geo.F = F; ctx.geo.n_fft = 2; ctx.geo.log2n = 1; ctx.geo.hop = 1; ctx.geo.pad = 0;
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&ctx.sm_count, cudaDevAttrMultiProcessorCount, dev);
-  if (e != cudaSuccess) return cuda_fail(e, "setk_cgmm_stft(device)");
-  return with_bin_major(stft, B, C, F, T, cgmm_workspace_bytes(&ctx, B, T, num_classes, bin_pitch(F)), stream,
-                        "setk_cgmm_stft(workspace)", "setk_cgmm_stft", [&](float2* X, int P, double* ws) {
-    return run_cgmm(&ctx, X, P, ws, nullptr, B, /*N=*/T + 1, T, num_classes, num_iters, init_gamma, update_alpha,
-                    masks, status, stream);
-  });
-}
-
 // plan rows (iterations, lo, hi) of the permutation aligner: 0 <= lo < hi <= F, iterations >= 0;
 // NULL or R = 0 (no alignment) only when `required` is false
 static int check_permu_plan(const char* who, const int32_t* plan, int R, int F, bool required) {
@@ -581,68 +525,113 @@ static int check_permu_plan(const char* who, const int32_t* plan, int R, int F, 
   return SETK_OK;
 }
 
-// the checks every CACGMM / alignment entry point shares: class count, start, plan rows over F bins
-static int check_cacgmm(const char* who, int C, int K, int num_iters, const double* init_gamma, int cgmm_init,
-                        const int32_t* plan, int R, int F) {
+// the model arguments every CGMM / CACGMM entry point refuses: class count, channels, start, iterations and
+// plan rows over F bins
+static int check_em(const char* who, const CgmmModel& m, int C, int F, int K, int num_iters) {
   if (K < 2 || K > 4) return fail(SETK_EINVAL, "%s: num_classes %d outside 2..4", who, K);
-  if (C < 2) return fail(SETK_EINVAL, "%s: %d channel(s), the CACGMM needs 2 or more", who, C);
+  if (m.acg && C < 2) return fail(SETK_EINVAL, "%s: %d channel(s), the CACGMM needs 2 or more", who, C);
+  if (!m.acg && !m.gamma32 && K != 2)
+    return fail(SETK_EINVAL, "%s: %d classes need init_gamma (the reference's start is random)", who, K);
   if (num_iters < 0) return fail(SETK_EINVAL, "%s: num_iters %d", who, num_iters);
-  if (!init_gamma && !(cgmm_init && K == 2))
+  if (m.acg && !m.gamma64 && !(m.cgmm_init && K == 2))
     return fail(SETK_EINVAL, "%s: a NULL init_gamma needs cgmm_init with 2 classes", who);
-  return check_permu_plan(who, plan, R, F, false);
+  return check_permu_plan(who, m.permu_rows, m.R, F, false);
+}
+
+// the geometry of a call that gives its frames rather than samples: the frame count never limits
+static Geometry frames_given(int C, int F) {
+  Geometry g;
+  g.C = C; g.F = F; g.n_fft = 2; g.log2n = 1; g.hop = 1; g.pad = 0;
+  return g;
+}
+
+// what the EM passes need of a plan, for a call without one: frames_given and the device's SM count
+static cudaError_t plan_free_ctx(int C, int F, CgCtx* ctx) {
+  ctx->geo = frames_given(C, F);
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, dev);
+  return e;
+}
+
+// setk_cgmm_masks / setk_cacgmm_masks: the tile STFT of the plan's audio, then the EM run of model m
+static int em_masks(const char* who, const CgmmModel& m, setk_plan_t* pl, const float* audio,
+                    const int32_t* n_samples, int B, int N, int K, int num_iters, float* masks, unsigned* status,
+                    void* stream) {
+  int rc = check_batch(pl, B, N, who);
+  if (rc) return rc;
+  if (!audio || !masks) return fail(SETK_EINVAL, "%s: null buffer", who);
+  const Geometry& g = pl->geo;
+  rc = check_em(who, m, g.C, g.F, K, num_iters);
+  if (rc) return rc;
+  if (!stft_spill_supported(g))
+    return fail(SETK_EUNSUPPORTED, "%s: needs n_fft 512 or 1024 (got %d, hop %d)", who, g.n_fft, g.hop);
+  const int T = frames_of(N, g.n_fft, g.hop, g.pad);
+  if (T < 1) return fail(SETK_ESHAPE, "%s: no frame in %d samples", who, N);
+  if (m.R > 0 && permu_scratch_bytes(B, K, T, g.F) < 0)
+    return fail(SETK_EUNSUPPORTED, "%s: %d bins exceed the aligner's shared memory", who, g.F);
+  char ws_what[64];
+  snprintf(ws_what, sizeof(ws_what), "%s(workspace)", who);
+  const int P = bin_pitch(g.F);
+  CgCtx ctx;
+  ctx.geo = g; ctx.sm_count = pl->sm_count;
+  cudaError_t e = ensure(&pl->d_cgmm_ws, &pl->cgmm_ws_bytes, cgmm_workspace_bytes(&ctx, m, B, T, K, P));
+  if (e != cudaSuccess) return cuda_fail(e, ws_what);
+  rc = stft_to_bin_major(pl, audio, n_samples, B, N, T, nullptr, stream, ws_what, who);
+  if (rc) return rc;
+  e = run_cgmm(&ctx, m, pl->d_stft_ws, P, pl->d_cgmm_ws, n_samples, B, N, T, K, num_iters, masks, status, stream);
+  return done(e, who);
+}
+
+// setk_cgmm_stft / setk_cacgmm_stft: the EM run of model m over a caller's [B][C][F][T] STFT
+static int em_stft(const char* who, const CgmmModel& m, const void* stft, int B, int C, int F, int T, int K,
+                   int num_iters, float* masks, unsigned* status, void* stream) {
+  if (!stft || !masks) return fail(SETK_EINVAL, "%s: null buffer", who);
+  if (B < 1 || B > 65535 || F < 1 || T < 1 || C < 1 || C > SETK_MAX_CHANNELS)
+    return fail(SETK_ESHAPE, "%s: bad shape B=%d C=%d F=%d T=%d", who, B, C, F, T);
+  int rc = check_em(who, m, C, F, K, num_iters);
+  if (rc) return rc;
+  if (m.R > 0 && permu_scratch_bytes(B, K, T, F) < 0)
+    return fail(SETK_EUNSUPPORTED, "%s: %d bins exceed the aligner's shared memory", who, F);
+  char dev_what[64], ws_what[64];
+  snprintf(dev_what, sizeof(dev_what), "%s(device)", who);
+  snprintf(ws_what, sizeof(ws_what), "%s(workspace)", who);
+  CgCtx ctx;
+  cudaError_t e = plan_free_ctx(C, F, &ctx);
+  if (e != cudaSuccess) return cuda_fail(e, dev_what);
+  return with_bin_major(stft, B, C, F, T, cgmm_workspace_bytes(&ctx, m, B, T, K, bin_pitch(F)), stream, ws_what, who,
+                        [&](float2* X, int P, double* ws) {
+    return run_cgmm(&ctx, m, X, P, ws, nullptr, B, /*N=*/T + 1, T, K, num_iters, masks, status, stream);
+  });
+}
+
+int setk_cgmm_masks(setk_plan_t* pl, const float* audio, const int32_t* n_samples, int32_t B, int32_t N,
+                    int32_t num_classes, int32_t num_iters, const float* init_gamma, int32_t update_alpha,
+                    float* masks, uint32_t* status, void* stream) {
+  const CgmmModel m = {false, init_gamma, nullptr, 0, update_alpha, nullptr, 0};
+  return em_masks("setk_cgmm_masks", m, pl, audio, n_samples, B, N, num_classes, num_iters, masks, status, stream);
+}
+
+int setk_cgmm_stft(const void* stft, int32_t B, int32_t C, int32_t F, int32_t T, int32_t num_classes,
+                   int32_t num_iters, const float* init_gamma, int32_t update_alpha, float* masks,
+                   uint32_t* status, void* stream) {
+  const CgmmModel m = {false, init_gamma, nullptr, 0, update_alpha, nullptr, 0};
+  return em_stft("setk_cgmm_stft", m, stft, B, C, F, T, num_classes, num_iters, masks, status, stream);
 }
 
 int setk_cacgmm_masks(setk_plan_t* pl, const float* audio, const int32_t* n_samples, int32_t B, int32_t N,
                       int32_t num_classes, int32_t num_iters, const double* init_gamma, int32_t cgmm_init,
                       int32_t update_alpha, const int32_t* permu_plan, int32_t R, float* masks, uint32_t* status,
                       void* stream) {
-  int rc = check_batch(pl, B, N, "setk_cacgmm_masks");
-  if (rc) return rc;
-  if (!audio || !masks) return fail(SETK_EINVAL, "setk_cacgmm_masks: null buffer");
-  const Geometry& g = pl->geo;
-  rc = check_cacgmm("setk_cacgmm_masks", g.C, num_classes, num_iters, init_gamma, cgmm_init, permu_plan, R, g.F);
-  if (rc) return rc;
-  if (!stft_spill_supported(g))
-    return fail(SETK_EUNSUPPORTED, "setk_cacgmm_masks: needs n_fft 512 or 1024 (got %d, hop %d)", g.n_fft, g.hop);
-  const int T = frames_of(N, g.n_fft, g.hop, g.pad);
-  if (T < 1) return fail(SETK_ESHAPE, "setk_cacgmm_masks: no frame in %d samples", N);
-  if (permu_plan && R > 0 && permu_scratch_bytes(B, num_classes, T, g.F) < 0)
-    return fail(SETK_EUNSUPPORTED, "setk_cacgmm_masks: %d bins exceed the aligner's shared memory", g.F);
-  const int P = bin_pitch(g.F);
-  CgCtx ctx;
-  ctx.geo = g; ctx.sm_count = pl->sm_count;
-  cudaError_t e = ensure(&pl->d_cgmm_ws, &pl->cgmm_ws_bytes, cacgmm_workspace_bytes(&ctx, B, T, num_classes, P));
-  if (e != cudaSuccess) return cuda_fail(e, "setk_cacgmm_masks(workspace)");
-  rc = stft_to_bin_major(pl, audio, n_samples, B, N, T, nullptr, stream, "setk_cacgmm_masks(workspace)",
-                         "setk_cacgmm_masks");
-  if (rc) return rc;
-  e = run_cacgmm(&ctx, pl->d_stft_ws, P, pl->d_cgmm_ws, n_samples, B, N, T, num_classes, num_iters, init_gamma,
-                 cgmm_init, update_alpha, permu_plan, permu_plan ? R : 0, masks, status, stream);
-  return done(e, "setk_cacgmm_masks");
+  const CgmmModel m = {true, nullptr, init_gamma, cgmm_init, update_alpha, permu_plan, permu_plan ? R : 0};
+  return em_masks("setk_cacgmm_masks", m, pl, audio, n_samples, B, N, num_classes, num_iters, masks, status, stream);
 }
 
 int setk_cacgmm_stft(const void* stft, int32_t B, int32_t C, int32_t F, int32_t T, int32_t num_classes,
                      int32_t num_iters, const double* init_gamma, int32_t cgmm_init, int32_t update_alpha,
                      const int32_t* permu_plan, int32_t R, float* masks, uint32_t* status, void* stream) {
-  if (!stft || !masks) return fail(SETK_EINVAL, "setk_cacgmm_stft: null buffer");
-  if (B < 1 || B > 65535 || F < 1 || T < 1 || C < 1 || C > SETK_MAX_CHANNELS)
-    return fail(SETK_ESHAPE, "setk_cacgmm_stft: bad shape B=%d C=%d F=%d T=%d", B, C, F, T);
-  int rc = check_cacgmm("setk_cacgmm_stft", C, num_classes, num_iters, init_gamma, cgmm_init, permu_plan, R, F);
-  if (rc) return rc;
-  if (permu_plan && R > 0 && permu_scratch_bytes(B, num_classes, T, F) < 0)
-    return fail(SETK_EUNSUPPORTED, "setk_cacgmm_stft: %d bins exceed the aligner's shared memory", F);
-  CgCtx ctx;
-  // frames are given, not derived from samples: a geometry whose frame count never limits
-  ctx.geo.C = C; ctx.geo.F = F; ctx.geo.n_fft = 2; ctx.geo.log2n = 1; ctx.geo.hop = 1; ctx.geo.pad = 0;
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&ctx.sm_count, cudaDevAttrMultiProcessorCount, dev);
-  if (e != cudaSuccess) return cuda_fail(e, "setk_cacgmm_stft(device)");
-  return with_bin_major(stft, B, C, F, T, cacgmm_workspace_bytes(&ctx, B, T, num_classes, bin_pitch(F)), stream,
-                        "setk_cacgmm_stft(workspace)", "setk_cacgmm_stft", [&](float2* X, int P, double* ws) {
-    return run_cacgmm(&ctx, X, P, ws, nullptr, B, /*N=*/T + 1, T, num_classes, num_iters, init_gamma, cgmm_init,
-                      update_alpha, permu_plan, permu_plan ? R : 0, masks, status, stream);
-  });
+  const CgmmModel m = {true, nullptr, init_gamma, cgmm_init, update_alpha, permu_plan, permu_plan ? R : 0};
+  return em_stft("setk_cacgmm_stft", m, stft, B, C, F, T, num_classes, num_iters, masks, status, stream);
 }
 
 int setk_permu_align(const double* masks, const int32_t* n_frames, int32_t B, int32_t K, int32_t T, int32_t F,
@@ -656,7 +645,7 @@ int setk_permu_align(const double* masks, const int32_t* n_frames, int32_t B, in
   if (sb < 0) return fail(SETK_EUNSUPPORTED, "setk_permu_align: %d bins exceed the aligner's shared memory", F);
   PermuArgs a;
   a.m = masks; a.ld = F; a.n_frames = n_frames; a.n_samples = nullptr; a.N = T + 1;
-  a.g.C = 1; a.g.F = F; a.g.n_fft = 2; a.g.log2n = 1; a.g.hop = 1; a.g.pad = 0;   // T frames unless n_frames
+  a.g = frames_given(1, F);   // T frames unless n_frames
   a.K = K; a.T = T; a.F = F;
   return with_scratch((size_t)sb + 256, stream, "setk_permu_align(scratch)", "setk_permu_align", [&](char* ws) {
     return run_permu_align(a, B, plan, R, reinterpret_cast<double*>(ws), out, mapping, stream);

@@ -572,13 +572,14 @@ static int cgmm_cov_chunks(const CgCtx* pl, int B, int T) {
   return chunks;
 }
 
-size_t cgmm_workspace_bytes(const CgCtx* pl, int B, int T, int K, int P) {
+size_t cgmm_workspace_bytes(const CgCtx* pl, const CgmmModel& m, int B, int T, int K, int P) {
   const Geometry& g = pl->geo;
   const int chunks = cgmm_cov_chunks(pl, B, T);
   size_t n = 2 * (size_t)B * K * T * P;                          // G, W
   n += (size_t)B * chunks * K * (g.C * g.C + 1) * g.F;           // part
   n += (size_t)B * K * g.C * g.C * g.F;                          // Rinv
   n += 2 * (size_t)B * K * g.F;                                  // logdet, alpha
+  if (m.acg) n += (size_t)B * K * T;                             // the aligner's centroids
   return n * sizeof(double);
 }
 
@@ -717,81 +718,65 @@ static cudaError_t cgmm_estep(const CgCtx* pl, const float2* X, int P, const Cgm
   }
 }
 
-// CgmmTrainer(...).train(num_iters) over the workspace X of B utterances.
-cudaError_t run_cgmm(const CgCtx* pl, const float2* X, int P, double* ws, const int* n_samples, int B, int N,
-                     int T, int K, int num_iters, const float* init_gamma, int update_alpha, float* masks,
-                     unsigned* status, void* stream) {
-  const Geometry& g = pl->geo;
-  const CgmmWorkspace w = cgmm_carve(pl, ws, B, T, K, P);
-  cudaError_t e;
-  {  // alpha = 1 / K  (cluster.py:447)
-    const long long n = (long long)B * K * g.F;
-    e = launch(cgmm_fill_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, stream, true, w.alpha, n,
-               1.0 / (double)K);
-    if (e != cudaSuccess) return e;
-  }
-  const bool uniform = init_gamma == nullptr;           // K = 2: R_0 = sum y y^H / T, R_1 = I
+// one pass over the workspace: covariance -> factor -> E-step
+static cudaError_t cgmm_pass(const CgCtx* pl, const CgmmModel& m, const float2* X, int P, const CgmmWorkspace& w,
+                             bool uniform, int identity_class, int update_alpha, const int* n_samples, int B, int N,
+                             int T, int K, unsigned* status, void* stream) {
+  cudaError_t e = cgmm_cov(pl, X, P, w, uniform, n_samples, B, N, T, K, stream);
+  if (e == cudaSuccess) e = cgmm_factor(pl, w, identity_class, update_alpha, n_samples, B, N, T, K, status, stream);
+  if (e != cudaSuccess) return e;
+  return m.acg ? cgmm_estep<true>(pl, X, P, w, n_samples, B, N, T, K, stream)
+               : cgmm_estep<false>(pl, X, P, w, n_samples, B, N, T, K, stream);
+}
+
+// CgmmTrainer start (cluster.py:436-447): the given posteriors, or with none (K = 2)
+// R_0 = sum y y^H / T, R_1 = I and one E-step
+static cudaError_t cgmm_start(const CgCtx* pl, const CgmmModel& m, const float2* X, int P, const CgmmWorkspace& w,
+                              const int* n_samples, int B, int N, int T, int K, unsigned* status, void* stream) {
+  const bool uniform = m.gamma32 == nullptr;
   if (!uniform) {
-    const long long n = (long long)B * K * T * g.F;
-    e = launch(cgmm_import_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, stream, true, init_gamma,
-               B, K, T, g.F, P, w.G, w.W);
+    const long long n = (long long)B * K * T * pl->geo.F;
+    cudaError_t e = launch(cgmm_import_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, stream, true,
+                           m.gamma32, B, K, T, pl->geo.F, P, w.G, w.W);
     if (e != cudaSuccess) return e;
   }
-  e = cgmm_cov(pl, X, P, w, uniform, n_samples, B, N, T, K, stream);
-  if (e == cudaSuccess) e = cgmm_factor(pl, w, uniform ? 1 : -1, 0, n_samples, B, N, T, K, status, stream);
-  if (e == cudaSuccess) e = cgmm_estep<false>(pl, X, P, w, n_samples, B, N, T, K, stream);
-  for (int it = 0; it < num_iters && e == cudaSuccess; ++it) {
-    e = cgmm_cov(pl, X, P, w, false, n_samples, B, N, T, K, stream);
-    if (e == cudaSuccess) e = cgmm_factor(pl, w, -1, update_alpha, n_samples, B, N, T, K, status, stream);
-    if (e == cudaSuccess) e = cgmm_estep<false>(pl, X, P, w, n_samples, B, N, T, K, stream);
-  }
-  if (e != cudaSuccess) return e;
-  const long long n = (long long)B * K * T * g.F;
-  return launch(cgmm_export_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, stream, true,
-                (const double*)w.G, n_samples, N, g, B, K, T, P, masks);
+  return cgmm_pass(pl, m, X, P, w, uniform, uniform ? 1 : -1, 0, n_samples, B, N, T, K, status, stream);
 }
 
-size_t cacgmm_workspace_bytes(const CgCtx* pl, int B, int T, int K, int P) {
-  return cgmm_workspace_bytes(pl, B, T, K, P) + sizeof(double) * (size_t)B * K * T;   // + aligner centroids
+// CacgmmTrainer start (cluster.py:495-518): the given posteriors, or with cgmm_init (K = 2)
+// B_0 = sum_t z z^H / T, B_1 = I and one E-step
+static cudaError_t cacgmm_start(const CgCtx* pl, const CgmmModel& m, const float2* X, int P, const CgmmWorkspace& w,
+                                const int* n_samples, int B, int N, int T, int K, unsigned* status, void* stream) {
+  const Geometry& g = pl->geo;
+  const bool from_cgmm = m.cgmm_init && K == 2;
+  const long long n = (long long)B * T * g.F;
+  cudaError_t e = launch(cacgmm_import_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, stream, true,
+                         from_cgmm ? nullptr : m.gamma64, X, P, g.C, B, K, T, g.F, w.G, w.W);
+  if (e != cudaSuccess || !from_cgmm) return e;
+  return cgmm_pass(pl, m, X, P, w, false, 1, 0, n_samples, B, N, T, K, status, stream);
 }
 
-// CacgmmTrainer(obs, K, gamma, cgmm_init=..., update_alpha=...).train(num_iters) (cluster.py:468-535)
-// over the workspace X, then permu_aligner (cluster.py:48-91) on the fp64 posteriors when R > 0.
-cudaError_t run_cacgmm(const CgCtx* pl, const float2* X, int P, double* ws, const int* n_samples, int B, int N,
-                       int T, int K, int num_iters, const double* init_gamma, int cgmm_init, int update_alpha,
-                       const int* permu_rows, int R, float* masks, unsigned* status, void* stream) {
+// CgmmTrainer / CacgmmTrainer(...).train(num_iters) (cluster.py:396-465, 468-535) over the workspace X
+// of B utterances, then the masks, or permu_aligner (cluster.py:48-91) on the fp64 posteriors when
+// m.R > 0.
+cudaError_t run_cgmm(const CgCtx* pl, const CgmmModel& m, const float2* X, int P, double* ws, const int* n_samples,
+                     int B, int N, int T, int K, int num_iters, float* masks, unsigned* status, void* stream) {
   const Geometry& g = pl->geo;
   const CgmmWorkspace w = cgmm_carve(pl, ws, B, T, K, P);
-  cudaError_t e;
-  {  // alpha = 1 / K  (cluster.py:485)
-    const long long n = (long long)B * K * g.F;
-    e = launch(cgmm_fill_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, stream, true, w.alpha, n,
-               1.0 / (double)K);
-    if (e != cudaSuccess) return e;
-  }
-  const bool from_cgmm = cgmm_init && K == 2;
-  {
-    const long long n = (long long)B * T * g.F;
-    e = launch(cacgmm_import_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, stream, true,
-               from_cgmm ? nullptr : init_gamma, X, P, g.C, B, K, T, g.F, w.G, w.W);
-    if (e != cudaSuccess) return e;
-  }
-  if (from_cgmm) {   // B_0 = sum_t z z^H / T, B_1 = I, then one E-step (cluster.py:495-506)
-    e = cgmm_cov(pl, X, P, w, false, n_samples, B, N, T, K, stream);
-    if (e == cudaSuccess) e = cgmm_factor(pl, w, 1, 0, n_samples, B, N, T, K, status, stream);
-    if (e == cudaSuccess) e = cgmm_estep<true>(pl, X, P, w, n_samples, B, N, T, K, stream);
-  }
-  for (int it = 0; it < num_iters && e == cudaSuccess; ++it) {
-    e = cgmm_cov(pl, X, P, w, false, n_samples, B, N, T, K, stream);
-    if (e == cudaSuccess) e = cgmm_factor(pl, w, -1, update_alpha, n_samples, B, N, T, K, status, stream);
-    if (e == cudaSuccess) e = cgmm_estep<true>(pl, X, P, w, n_samples, B, N, T, K, stream);
-  }
+  const long long na = (long long)B * K * g.F;         // alpha = 1 / K  (cluster.py:447, 485)
+  cudaError_t e = launch(cgmm_fill_kernel, dim3((unsigned)((na + 255) / 256)), dim3(256), 0, stream, true,
+                         w.alpha, na, 1.0 / (double)K);
+  if (e == cudaSuccess)
+    e = m.acg ? cacgmm_start(pl, m, X, P, w, n_samples, B, N, T, K, status, stream)
+              : cgmm_start(pl, m, X, P, w, n_samples, B, N, T, K, status, stream);
+  for (int it = 0; it < num_iters && e == cudaSuccess; ++it)
+    e = cgmm_pass(pl, m, X, P, w, false, -1, m.update_alpha, n_samples, B, N, T, K, status, stream);
   if (e != cudaSuccess) return e;
-  if (R > 0) {
+  if (m.R > 0) {
     PermuArgs a;
     a.m = w.G; a.ld = P; a.n_frames = nullptr; a.n_samples = n_samples; a.N = N; a.g = g;
     a.K = K; a.T = T; a.F = g.F;
-    return run_permu_align(a, B, permu_rows, R, w.alpha + (size_t)B * K * g.F, masks, nullptr, stream);
+    return run_permu_align(a, B, m.permu_rows, m.R, w.alpha + (size_t)B * K * g.F, masks, nullptr, stream);
   }
   const long long n = (long long)B * K * T * g.F;
   return launch(cgmm_export_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, stream, true,

@@ -87,17 +87,19 @@ cudaError_t weights_coop_launch(const WeightsArgs& a, int C, void* stream);
 cudaError_t post_run(int mode, const void* A, const void* Rn, int dtype, int B, int F, int C, void* out,
                      unsigned* status, void* stream);
 
-// ---- cgmm.cu: CGMM mask estimation over a bin-major STFT ----
-struct CgCtx { Geometry geo; int sm_count; };   // what the CGMM passes need of a plan
+// ---- cgmm.cu: CGMM and CACGMM mask estimation over a bin-major STFT ----
+struct CgCtx { Geometry geo; int sm_count; };   // what the EM passes need of a plan
+struct CgmmModel {                               // what one EM run's model needs beyond the passes
+  bool acg;                        // CACGMM on the unit-norm observations; else CGMM
+  const float* gamma32;            // CGMM start [B][K][T][F], or null: the K = 2 start
+  const double* gamma64;           // CACGMM start [B][K][T][F], or null with cgmm_init and K = 2
+  int cgmm_init, update_alpha;
+  const int* permu_rows; int R;    // host aligner plan rows (CACGMM); R = 0 exports the posteriors
+};
 cudaError_t run_bcft_to_spill(const float2* in, int B, int C, int F, int T, int P, float2* xws, void* stream);
-size_t cgmm_workspace_bytes(const CgCtx* pl, int B, int T, int K, int P);
-cudaError_t run_cgmm(const CgCtx* pl, const float2* X, int P, double* ws, const int* n_samples, int B, int N,
-                     int T, int K, int num_iters, const float* init_gamma, int update_alpha, float* masks,
-                     unsigned* status, void* stream);
-size_t cacgmm_workspace_bytes(const CgCtx* pl, int B, int T, int K, int P);
-cudaError_t run_cacgmm(const CgCtx* pl, const float2* X, int P, double* ws, const int* n_samples, int B, int N,
-                       int T, int K, int num_iters, const double* init_gamma, int cgmm_init, int update_alpha,
-                       const int* permu_rows, int R, float* masks, unsigned* status, void* stream);
+size_t cgmm_workspace_bytes(const CgCtx* pl, const CgmmModel& m, int B, int T, int K, int P);
+cudaError_t run_cgmm(const CgCtx* pl, const CgmmModel& m, const float2* X, int P, double* ws, const int* n_samples,
+                     int B, int N, int T, int K, int num_iters, float* masks, unsigned* status, void* stream);
 
 // ---- permu.cu: frequency permutation alignment of K-class masks ----
 struct PermuArgs {

@@ -113,7 +113,28 @@ def _complex_obs(obs, who):
     return obs.to(dev).to(torch.complex64).contiguous(), numpy, batched
 
 
-class CgmmTrainer(object):
+class _EmTrainer(object):
+    """train() of CgmmTrainer and CacgmmTrainer; each gives _run(num_iters) -> (masks, status), _model and
+    _diverged, the exception of an eigen-iteration that does not converge."""
+
+    def train(self, num_iters):
+        """
+        EM iterations; returns the posteriors K x F x T.  Calling it again continues: the run is
+        deterministic, so it is redone with the accumulated count.
+        """
+        self._iters += int(num_iters)
+        masks, status = self._run(self._iters)
+        bad = status.nonzero().flatten().tolist()
+        if bad:
+            raise self._diverged(f"{self._model}: eigen-iteration did not converge for batch entries {bad}")
+        gamma = masks.transpose(-1, -2)                              # K x F x T like the reference
+        if not self._batched:
+            gamma = gamma[0]
+        self.gamma = gamma.cpu().numpy() if self._numpy else gamma
+        return self.gamma
+
+
+class CgmmTrainer(_EmTrainer):
     """
     CGMM trainer (cluster.py:396-465).
         obs    mixture STFT, M x F x T complex (or B x M x F x T for a batch)
@@ -148,25 +169,14 @@ class CgmmTrainer(object):
         self._iters = 0
         self.gamma = None
 
-    def train(self, num_iters):
-        """
-        EM iterations; returns the posteriors K x F x T.  Calling it again continues:
-        the run is deterministic, so it is redone with the accumulated count.
-        """
-        self._iters += int(num_iters)
-        masks, status = _plan.cgmm_from_stft(self.obs, self.num_classes, self._iters,
-                                             init_gamma=self._init, update_alpha=self.update_alpha)
-        bad = status.nonzero().flatten().tolist()
-        if bad:
-            raise RuntimeError(f"CGMM: eigen-iteration did not converge for batch entries {bad}")
-        gamma = masks.transpose(-1, -2)                              # K x F x T like the reference
-        if not self._batched:
-            gamma = gamma[0]
-        self.gamma = gamma.cpu().numpy() if self._numpy else gamma
-        return self.gamma
+    _model, _diverged = "CGMM", RuntimeError
+
+    def _run(self, num_iters):
+        return _plan.cgmm_from_stft(self.obs, self.num_classes, num_iters, init_gamma=self._init,
+                                    update_alpha=self.update_alpha)
 
 
-class CacgmmTrainer(object):
+class CacgmmTrainer(_EmTrainer):
     """
     CACGMM trainer (cluster.py:468-535).
         obs        mixture STFT, M x F x T complex (or B x M x F x T for a batch)
@@ -206,19 +216,8 @@ class CacgmmTrainer(object):
         self._iters = 0
         self.gamma = None
 
-    def train(self, num_iters):
-        """
-        EM iterations; returns the posteriors K x F x T.  Calling it again continues: the run is
-        deterministic, so it is redone with the accumulated count.
-        """
-        self._iters += int(num_iters)
-        masks, status = _plan.cacgmm_from_stft(self.obs, self.num_classes, self._iters, init_gamma=self._init,
-                                               cgmm_init=self.cgmm_init, update_alpha=self.update_alpha)
-        bad = status.nonzero().flatten().tolist()
-        if bad:
-            raise np.linalg.LinAlgError(f"CACGMM: eigen-iteration did not converge for batch entries {bad}")
-        gamma = masks.transpose(-1, -2)                              # K x F x T like the reference
-        if not self._batched:
-            gamma = gamma[0]
-        self.gamma = gamma.cpu().numpy() if self._numpy else gamma
-        return self.gamma
+    _model, _diverged = "CACGMM", np.linalg.LinAlgError
+
+    def _run(self, num_iters):
+        return _plan.cacgmm_from_stft(self.obs, self.num_classes, num_iters, init_gamma=self._init,
+                                      cgmm_init=self.cgmm_init, update_alpha=self.update_alpha)

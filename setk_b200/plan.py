@@ -98,6 +98,15 @@ def _launch(dev, name, *args):
         _lib.check(getattr(_lib.library(), name)(*args, _lib.current_stream(dev)))
 
 
+def _em_masks(dev, name, B, K, T, F, *args):
+    """Allocates masks (B,K,T,F) float32 and status (B,) int32 on `dev`, launches `name`(*args, masks, status)
+    and returns (masks, status)."""
+    masks = torch.empty((B, K, T, F), dtype=torch.float32, device=dev)
+    status = torch.zeros((B,), dtype=torch.int32, device=dev)
+    _launch(dev, name, *args, _lib.ptr(masks), _lib.ptr(status))
+    return masks, status
+
+
 class StftPlan(object):
     """
     One STFT geometry (mirrors StftParser, libs/opts.py:21-49, and the keyword
@@ -251,11 +260,8 @@ class StftPlan(object):
         K = int(num_classes)
         init_gamma = _arg(init_gamma, self.device, torch.float32, (B, K, T, F), "init_gamma")
         ns = _arg(n_samples, self.device, torch.int32, (B,), "n_samples")
-        masks = torch.empty((B, K, T, F), dtype=torch.float32, device=self.device)
-        status = torch.zeros((B,), dtype=torch.int32, device=self.device)
-        _launch(self.device, "setk_cgmm_masks", self._h, _lib.ptr(audio), _lib.ptr(ns), B, N, K, int(num_iters),
-                _lib.ptr(init_gamma), 1 if update_alpha else 0, _lib.ptr(masks), _lib.ptr(status))
-        return masks, status
+        return _em_masks(self.device, "setk_cgmm_masks", B, K, T, F, self._h, _lib.ptr(audio), _lib.ptr(ns), B, N, K,
+                         int(num_iters), _lib.ptr(init_gamma), 1 if update_alpha else 0)
 
     def cacgmm_masks(self, audio, num_classes=2, num_iters=50, init_gamma=None, cgmm_init=False,
                      update_alpha=True, permu_plan=None, n_samples=None):
@@ -272,12 +278,9 @@ class StftPlan(object):
         K, rows, rows_p, R = _cacgmm_checks(C, num_classes, num_iters, init_gamma, cgmm_init, permu_plan, F)
         init_gamma = _arg(init_gamma, self.device, torch.float64, (B, K, T, F), "init_gamma")
         ns = _arg(n_samples, self.device, torch.int32, (B,), "n_samples")
-        masks = torch.empty((B, K, T, F), dtype=torch.float32, device=self.device)
-        status = torch.zeros((B,), dtype=torch.int32, device=self.device)
-        _launch(self.device, "setk_cacgmm_masks", self._h, _lib.ptr(audio), _lib.ptr(ns), B, N, K, int(num_iters),
-                _lib.ptr(init_gamma), int(bool(cgmm_init)), int(bool(update_alpha)), rows_p, R, _lib.ptr(masks),
-                _lib.ptr(status))
-        return masks, status
+        return _em_masks(self.device, "setk_cacgmm_masks", B, K, T, F, self._h, _lib.ptr(audio), _lib.ptr(ns), B, N,
+                         K, int(num_iters), _lib.ptr(init_gamma), int(bool(cgmm_init)), int(bool(update_alpha)),
+                         rows_p, R)
 
     def istft(self, enh, n_out=None, norm=None):
         """enh (B,F,T) complex64 -> wave (B,n_out) float32 (inverse_stft)."""
@@ -324,11 +327,8 @@ def cgmm_from_stft(stft, num_classes=2, num_iters=20, init_gamma=None, update_al
     B, C, F, T = stft.shape
     K = int(num_classes)
     init_gamma = _arg(init_gamma, stft.device, torch.float32, (B, K, T, F), "init_gamma")
-    masks = torch.empty((B, K, T, F), dtype=torch.float32, device=stft.device)
-    status = torch.zeros((B,), dtype=torch.int32, device=stft.device)
-    _launch(stft.device, "setk_cgmm_stft", _lib.ptr(stft), B, C, F, T, K, int(num_iters), _lib.ptr(init_gamma),
-            1 if update_alpha else 0, _lib.ptr(masks), _lib.ptr(status))
-    return masks, status
+    return _em_masks(stft.device, "setk_cgmm_stft", B, K, T, F, _lib.ptr(stft), B, C, F, T, K, int(num_iters),
+                     _lib.ptr(init_gamma), 1 if update_alpha else 0)
 
 
 # frequency sub-band schedule of the permutation aligner, per number of bins: rows of (iterations,
@@ -384,11 +384,8 @@ def cacgmm_from_stft(stft, num_classes=2, num_iters=50, init_gamma=None, cgmm_in
     B, C, F, T = stft.shape
     K, rows, rows_p, R = _cacgmm_checks(C, num_classes, num_iters, init_gamma, cgmm_init, permu_plan, F)
     init_gamma = _arg(init_gamma, stft.device, torch.float64, (B, K, T, F), "init_gamma")
-    masks = torch.empty((B, K, T, F), dtype=torch.float32, device=stft.device)
-    status = torch.zeros((B,), dtype=torch.int32, device=stft.device)
-    _launch(stft.device, "setk_cacgmm_stft", _lib.ptr(stft), B, C, F, T, K, int(num_iters), _lib.ptr(init_gamma),
-            int(bool(cgmm_init)), int(bool(update_alpha)), rows_p, R, _lib.ptr(masks), _lib.ptr(status))
-    return masks, status
+    return _em_masks(stft.device, "setk_cacgmm_stft", B, K, T, F, _lib.ptr(stft), B, C, F, T, K, int(num_iters),
+                     _lib.ptr(init_gamma), int(bool(cgmm_init)), int(bool(update_alpha)), rows_p, R)
 
 
 def permu_align(masks, n_frames=None, plan=None):
