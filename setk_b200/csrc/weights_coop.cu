@@ -17,11 +17,13 @@
 
 namespace setk {
 
-#ifdef SETK_EMU
-template <int C> struct WCfg { static constexpr int THREADS = 32; };   // one warp: groups still share barriers
-#else
+// The CPU execution model (tests/emu) launches the same CTAs: several warps' groups share one CTA's
+// shared memory there too, and its warps run unsynchronised like the device's.  Inside one warp the
+// groups run in lock step, so a group that wrote past its slot would only reach a neighbour's A once
+// that A is dead; across warps it can land while the neighbour still uses it.  Whether it does
+// depends on how the warps interleave, on the device and on the emulator's threads alike, which is
+// why tests/solve_cases.py's batch-invariance check alternates fast and slow warps.
 template <int C> struct WCfg { static constexpr int THREADS = C <= 8 ? 128 : 64; };
-#endif
 
 __device__ __forceinline__ cd load_c(const void* base, int dtype, long long i) {
   if (dtype == SETK_C128) {
